@@ -251,8 +251,9 @@ __global__ void __launch_bounds__(kThreads, 2) fsr_fused_kernel(const __grid_con
           if (in) {
             const float ppx_full = easu_pos(x, a.c0x, a.c0z), ppy_full = easu_pos(y, a.c0y, a.c0w);
             const float fpx = floorf(ppx_full), fpy = floorf(ppy_full);
-            if constexpr (kStrict) c = easu_filter<TW>(sC, sF, (int)fpx - tx0, (int)fpy - sy0, ppx_full - fpx, ppy_full - fpy);
-            else c = easu_filter_fast<TW>(sC, sF, (int)fpx - tx0, (int)fpy - sy0, ppx_full - fpx, ppy_full - fpy);
+            const int o = ((int)fpy - sy0) * TW + (int)fpx - tx0;
+            if constexpr (kStrict) c = easu_filter<TW>(sC + o, sF + o, ppx_full - fpx, ppy_full - fpy);
+            else c = easu_filter_fast<TW>(sC + o, sF + o, ppx_full - fpx, ppy_full - fpy);
           } else {
             c = easu_bilinear(sC, TW, sColAxis[x - ex0], sRowAxis[y - ey0]);
           }

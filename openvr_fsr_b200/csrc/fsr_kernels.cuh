@@ -98,18 +98,27 @@ __device__ __forceinline__ void easu_tap_ref(float &aR, float &aG, float &aB, fl
   aW += w;
 }
 
-// FsrEasuF, ffx_fsr1.h:315-437, for the output pixel whose 'f' texel sits at tile coords (ix,iy)
-// with sub-texel phase (ppx,ppy).  sC = decoded colours (xyz), sF = per-texel features.
+// FsrEasuF, ffx_fsr1.h:315-437, for the output pixel whose 'f' texel is cf in the colour tile and fr in the feature
+// tile, with sub-texel phase (ppx,ppy) >= +0.
+//
+// Two kinds of reference additions are left out, because they can only change the sign of a zero that is then
+// squared:
+//  * the zero the feature sums start from (0 + p = p except p = -0).  Each len term is lenX or lenY (saturated, >= +0)
+//    times a bilinear weight (>= +0), never -0, so len has the same bits.  dirX / dirY can differ only in the sign of a
+//    zero.  After the normalisation (x dirR > 0, or 1 when both are below 1/32768) they reach the output only through
+//    squares, fabsf, and the products off*dir.  Those products are summed into vx / vy, which differ at most in the
+//    sign of a zero and are squared into d2.  A NaN or inf operand gives the same NaN either way.
+//  * 0 - pp for the tap offset 0: -pp differs only for pp = +0, and then off*dir is a zero that feeds vx / vy as above.
+// The colour and weight sums still start from zero: their sign can reach the output.
 template <int TW>
-__device__ __forceinline__ float3 easu_filter(const float4 *__restrict__ sC, const float4 *__restrict__ sF, int ix, int iy,
-                                              float ppx, float ppy) {
+__device__ __forceinline__ float3 easu_filter(const float4 *__restrict__ cf, const float4 *__restrict__ fr, float ppx,
+                                              float ppy) {
   // direction + length: bilinear blend of the four corner features (:380-386)
-  const float4 *fr = sF + iy * TW + ix;
   const float4 Ff = fr[0], Fg = fr[1], Fj = fr[TW], Fk = fr[TW + 1];
   const float qx = 1.0f - ppx, qy = 1.0f - ppy;
   const float wf = qx * qy, wg = ppx * qy, wj = qx * ppy, wk = ppx * ppy;
-  float dirX = 0.0f, dirY = 0.0f, len = 0.0f;
-  dirX += Ff.x * wf; len += Ff.z * wf; dirY += Ff.y * wf; len += Ff.w * wf;
+  float dirX = Ff.x * wf, len = Ff.z * wf, dirY = Ff.y * wf;
+  len += Ff.w * wf;
   dirX += Fg.x * wg; len += Fg.z * wg; dirY += Fg.y * wg; len += Fg.w * wg;
   dirX += Fj.x * wj; len += Fj.z * wj; dirY += Fj.y * wj; len += Fj.w * wj;
   dirX += Fk.x * wk; len += Fk.z * wk; dirY += Fk.y * wk; len += Fk.w * wk;
@@ -134,8 +143,8 @@ __device__ __forceinline__ float3 easu_filter(const float4 *__restrict__ sC, con
 
   // the 4 distinct off.x / off.y values and their products with dir (shared by the 12 taps)
   const float ndirY = -dirY;
-  const float ox0 = -1.0f - ppx, ox1 = 0.0f - ppx, ox2 = 1.0f - ppx, ox3 = 2.0f - ppx;
-  const float oy0 = -1.0f - ppy, oy1 = 0.0f - ppy, oy2 = 1.0f - ppy, oy3 = 2.0f - ppy;
+  const float ox0 = -1.0f - ppx, ox1 = -ppx, ox2 = 1.0f - ppx, ox3 = 2.0f - ppx;
+  const float oy0 = -1.0f - ppy, oy1 = -ppy, oy2 = 1.0f - ppy, oy3 = 2.0f - ppy;
   const float xd0 = ox0 * dirX, xd1 = ox1 * dirX, xd2 = ox2 * dirX, xd3 = ox3 * dirX;
   const float xn0 = ox0 * ndirY, xn1 = ox1 * ndirY, xn2 = ox2 * ndirY, xn3 = ox3 * ndirY;
   const float yd0 = oy0 * dirY, yd1 = oy1 * dirY, yd2 = oy2 * dirY, yd3 = oy3 * dirY;
@@ -145,7 +154,7 @@ __device__ __forceinline__ float3 easu_filter(const float4 *__restrict__ sC, con
   //  e f g h
   //  i j k l
   //    n o
-  const float4 *r0 = sC + (iy - 1) * TW + ix;
+  const float4 *r0 = cf - TW;
   const float4 f = r0[TW], g = r0[TW + 1], j = r0[2 * TW], k = r0[2 * TW + 1];
   float aR = 0.0f, aG = 0.0f, aB = 0.0f, aW = 0.0f;
   // reference accumulation order (:423-434): b c i j f e k l h g o n   (index 0..3 <-> offset -1..2)
@@ -194,9 +203,8 @@ __device__ __forceinline__ void easu_acc(f2 &aRG, f2 &aBW, const float4 c, float
 }
 
 template <int TW>
-__device__ __forceinline__ float3 easu_filter_fast(const float4 *__restrict__ sC, const float4 *__restrict__ sF, int ix,
-                                                   int iy, float ppx, float ppy) {
-  const float4 *fr = sF + iy * TW + ix;
+__device__ __forceinline__ float3 easu_filter_fast(const float4 *__restrict__ cf, const float4 *__restrict__ fr, float ppx,
+                                                   float ppy) {
   const float4 Ff = fr[0], Fg = fr[1], Fj = fr[TW], Fk = fr[TW + 1];
   const float qx = 1.0f - ppx, qy = 1.0f - ppy;
   const f2 wt = mul2(make_float2(qx, ppx), bc(qy)), wb = mul2(make_float2(qx, ppx), bc(ppy)); // (wf,wg) (wj,wk)
@@ -240,7 +248,7 @@ __device__ __forceinline__ float3 easu_filter_fast(const float4 *__restrict__ sC
   //  e f g h
   //  i j k l
   //    n o
-  const float4 *r0 = sC + (iy - 1) * TW + ix;
+  const float4 *r0 = cf - TW;
   f2 aRG = bc(0.0f), aBW = bc(0.0f);
   {
     const float4 b = r0[0], c = r0[1];
@@ -494,17 +502,24 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
         const float ppx_full = easu_pos(x, a.c0x, a.c0z);
         const float fpx = floorf(ppx_full);
         const float ppx = ppx_full - fpx;
-        const int ix = (int)fpx - tx0;
+        const int ix = (int)fpx - tx0 - sy0 * TW; // tile offset of texel (fpx, 0)
+        const int yEnd = min(yFirst + 16, a.dst.h);
+        // pitched target: the store address advances by two rows per pixel instead of being formed from (x, y)
+        uint8_t *out = a.dst.ptr + (size_t)yFirst * a.dst.pitch + (size_t)x * sizeof(texel_t<FOUT>);
 #pragma unroll 2
-        for (int k = 0; k < 8; ++k) {
-          const int y = yFirst + 2 * k;
-          if (y >= a.dst.h) break;
+        for (int y = yFirst; y < yEnd; y += 2) {
           const float ppy_full = easu_pos(y, a.c0y, a.c0w);
           const float fpy = floorf(ppy_full);
+          const int o = (int)fpy * TW + ix;
           float3 c;
-          if constexpr (kStrict) c = easu_filter<TW>(sC, sF, ix, (int)fpy - sy0, ppx, ppy_full - fpy);
-          else c = easu_filter_fast<TW>(sC, sF, ix, (int)fpy - sy0, ppx, ppy_full - fpy);
-          put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
+          if constexpr (kStrict) c = easu_filter<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
+          else c = easu_filter_fast<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
+          if constexpr (ANYIO) {
+            put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
+          } else {
+            *reinterpret_cast<texel_t<FOUT> *>(out) = encode_opaque<FOUT>(c.x, c.y, c.z);
+            out += 2 * (size_t)a.dst.pitch;
+          }
         }
       } else {
         const BilinAxis ax = easu_bilinear_axis(x, a.radW, a.src.w, tx0, cols);
@@ -552,15 +567,31 @@ __device__ __forceinline__ float3 rcas_filter(const float4 b, const float4 d, co
   const float mn4G = fminf(fminf(b.y, fminf(d.y, f.y)), h.y), mx4G = fmaxf(fmaxf(b.y, fmaxf(d.y, f.y)), h.y);
   const float mn4B = fminf(fminf(b.z, fminf(d.z, f.z)), h.z), mx4B = fmaxf(fmaxf(b.z, fmaxf(d.z, f.z)), h.z);
   // limiters need full-precision reciprocals (:748-755)
-  const float hitMinR = mn4R * rcp_mode_rcas<U8>(4.0f * mx4R);
-  const float hitMinG = mn4G * rcp_mode_rcas<U8>(4.0f * mx4G);
-  const float hitMinB = mn4B * rcp_mode_rcas<U8>(4.0f * mx4B);
-  const float hitMaxR = (1.0f - mx4R) * rcp_mode_rcas<U8>(4.0f * mn4R + (-4.0f));
-  const float hitMaxG = (1.0f - mx4G) * rcp_mode_rcas<U8>(4.0f * mn4G + (-4.0f));
-  const float hitMaxB = (1.0f - mx4B) * rcp_mode_rcas<U8>(4.0f * mn4B + (-4.0f));
-  const float lobeR = fmaxf(-hitMinR, hitMaxR), lobeG = fmaxf(-hitMinG, hitMaxG), lobeB = fmaxf(-hitMinB, hitMaxB);
-  const float lobe =
-      fmaxf((float)(-(0.25 - (1.0 / 16.0))), fminf(fmaxf(lobeR, fmaxf(lobeG, lobeB)), 0.0f)) * sharp;
+  float lobe;
+  if constexpr (U8) {
+    // UNORM8 source: the limiter with its factors of 4 taken out, the same bits.  With mx, mn in {k/255} nothing here
+    // is subnormal, so x4 and /4 are exact and commute with every rounding: fl(4mn-4) = 4 fl(mn-1) (fl(4mn) is exact),
+    // 1/(4x) = (1/x)/4, so each hitMin / hitMax / lobe and the clamped max below are exactly 4x the reference's; the
+    // x0.25 restores the reference's value BEFORE x sharp, so no assumption on `sharp` is needed.  Exhaustive host
+    // check over every (mn, mx) code pair with mn <= mx: tests/test_rcas_limiter_host.py.
+    const float hitMinR = mn4R * rcp_rn_unorm8_operand(mx4R);
+    const float hitMinG = mn4G * rcp_rn_unorm8_operand(mx4G);
+    const float hitMinB = mn4B * rcp_rn_unorm8_operand(mx4B);
+    const float hitMaxR = (1.0f - mx4R) * rcp_rn_unorm8_operand(mn4R + (-1.0f));
+    const float hitMaxG = (1.0f - mx4G) * rcp_rn_unorm8_operand(mn4G + (-1.0f));
+    const float hitMaxB = (1.0f - mx4B) * rcp_rn_unorm8_operand(mn4B + (-1.0f));
+    const float lobeR = fmaxf(-hitMinR, hitMaxR), lobeG = fmaxf(-hitMinG, hitMaxG), lobeB = fmaxf(-hitMinB, hitMaxB);
+    lobe = fmaxf((float)(-4.0 * (0.25 - (1.0 / 16.0))), fminf(fmaxf(lobeR, fmaxf(lobeG, lobeB)), 0.0f)) * 0.25f * sharp;
+  } else {
+    const float hitMinR = mn4R * rcp_mode(4.0f * mx4R);
+    const float hitMinG = mn4G * rcp_mode(4.0f * mx4G);
+    const float hitMinB = mn4B * rcp_mode(4.0f * mx4B);
+    const float hitMaxR = (1.0f - mx4R) * rcp_mode(4.0f * mn4R + (-4.0f));
+    const float hitMaxG = (1.0f - mx4G) * rcp_mode(4.0f * mn4G + (-4.0f));
+    const float hitMaxB = (1.0f - mx4B) * rcp_mode(4.0f * mn4B + (-4.0f));
+    const float lobeR = fmaxf(-hitMinR, hitMaxR), lobeG = fmaxf(-hitMinG, hitMaxG), lobeB = fmaxf(-hitMinB, hitMaxB);
+    lobe = fmaxf((float)(-(0.25 - (1.0 / 16.0))), fminf(fmaxf(lobeR, fmaxf(lobeG, lobeB)), 0.0f)) * sharp;
+  }
   const float rcpL = prx_med_rcp(4.0f * lobe + 1.0f);
   return make_float3((lobe * b.x + lobe * d.x + lobe * h.x + lobe * f.x + e.x) * rcpL,
                      (lobe * b.y + lobe * d.y + lobe * h.y + lobe * f.y + e.y) * rcpL,
@@ -676,7 +707,7 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       for (int q = tid; q < kRcasTH * (kTileW + 2); q += kThreads) {
         const int ty = q / (kTileW + 2), tx = q - ty * (kTileW + 2);
         float4 c = decode_rgba<FIN>(sRaw[ty * kRcasRawW + tx + 3]);
-        if constexpr (OPQ) c.w = 1.0f;
+        if constexpr (OPQ || PAIRED) c.w = 1.0f; // PAIRED: only the filter reads this tile, and it ignores alpha
         sC[ty * kRcasTW + tx] = c;
       }
   } else {
@@ -741,15 +772,19 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
   }
 }
 
-// Device self-test behind ovrfsr_selftest_rcp: every reciprocal operand strict RCAS can see with a UNORM8 source,
-// fast sequence vs rcp.rn.  out[0] = number of mismatching operands (must be 0), out[1] = operands checked.
+// Device self-test behind ovrfsr_selftest_rcp: every reciprocal operand strict RCAS can see with a UNORM8 source (mx
+// and mn-1), fast sequence vs rcp.rn; for the operand +0 the sequence must give the NaN the filter relies on.
+// out[0] = number of mismatching operands (must be 0), out[1] = operands checked.
+__device__ __forceinline__ bool rcp_unorm8_operand_ok(float x) {
+  const float r = rcp_rn_unorm8_operand(x);
+  return x == 0.0f ? isnan(r) : f2u(r) == f2u(__frcp_rn(x));
+}
 __global__ void rcas_rcp_selftest_kernel(uint32_t *out) {
   const int k = threadIdx.x; // 0..255
   const float v = unorm8((float)k);
-  const float x1 = 4.0f * v, x2 = __fadd_rn(__fmul_rn(4.0f, v), -4.0f);
   int bad = 0;
-  bad += f2u(rcp_rn_unorm8_operand(x1)) != f2u(__frcp_rn(x1));
-  bad += f2u(rcp_rn_unorm8_operand(x2)) != f2u(__frcp_rn(x2));
+  bad += !rcp_unorm8_operand_ok(v);
+  bad += !rcp_unorm8_operand_ok(__fadd_rn(v, -1.0f));
   atomicAdd(&out[0], (uint32_t)bad);
   atomicAdd(&out[1], 2u);
 }
