@@ -345,12 +345,41 @@ __device__ __forceinline__ float4 mid_roundtrip(float r, float g, float b) {
   }
 }
 
+// One-colour groups.  FsrEasuF ends in the de-ring clamp min(mx, max(mn, aC*rcp(aW))) with mn / mx over the four
+// nearest texels f, g, j, k.  Where those four have the same RGB, mn == mx == f and the clamp returns f whatever the
+// taps summed to: a finite v gives max(f, v) >= f and then min(f, .) == f, a NaN gives f (min / max ignore NaN).  A
+// decoded UNORM texel is a finite value >= +0 (no -0, no NaN), so such a pixel is exactly encode(f), in both math modes.
+// The footprint of a group -- every f / g / j / k any of its in-image pixels uses -- is the texel rectangle
+// floor(pos(first)) .. floor(pos(last)) + 1 in each axis (easu_pos is monotone).  Returns the tile offset of its first
+// texel when the whole rectangle has one RGB, else -1.  Tile coordinates: the tile is already clamped to the image edge.
+// Called by all 32 lanes of a warp: 16 columns x 2 rows per step, leaving at the first step that finds a second colour.
+template <int TW>
+__device__ __forceinline__ int easu_flat_group(const float4 *__restrict__ sC, const EasuArgs &a, int lane, int gx, int gy,
+                                               int tx0, int sy0) {
+  const int fx0 = (int)floorf(easu_pos(gx, a.c0x, a.c0z)) - tx0;
+  const int fx1 = (int)floorf(easu_pos(min(gx + 15, a.dst.w - 1), a.c0x, a.c0z)) + 1 - tx0;
+  const int fy0 = (int)floorf(easu_pos(gy, a.c0y, a.c0w)) - sy0;
+  const int fy1 = (int)floorf(easu_pos(min(gy + 15, a.dst.h - 1), a.c0y, a.c0w)) + 1 - sy0;
+  const float4 ref = sC[fy0 * TW + fx0];
+  for (int r = fy0; r <= fy1; r += 2) {
+    const int ty = r + (lane >> 4);
+    bool same = true;
+    for (int c = fx0; c <= fx1; c += 16) {
+      const int tx = c + (lane & 15);
+      if (ty <= fy1 && tx <= fx1) {
+        const float4 t = sC[ty * TW + tx];
+        same = same && f2u(t.x) == f2u(ref.x) && f2u(t.y) == f2u(ref.y) && f2u(t.z) == f2u(ref.z);
+      }
+    }
+    if (!__all_sync(0xFFFFFFFFu, same)) return -1;
+  }
+  return fy0 * TW + fx0;
+}
+
 // TW  = shared tile row stride in texels (compile time, so every tap is base + immediate): 60 covers out->in
 //       scales up to 0.81 for a 64-wide output tile (60 texels incl. the 4 TMA alignment columns), 72 the rest up to 1.0.
-// TMA = the raw RGBA8 source box (tile + halo) arrives by cp.async.bulk.tensor into a double-buffered landing zone
-//       and is decoded from there; otherwise (FP16/FP32 sources, unaligned pitch) texels are fetched with plain loads.
-// Persistent: the grid is (CTAs per SM) x (SM count); each CTA walks tiles t = blockIdx.x, +gridDim.x, ... in
-// row-major order and, in the TMA variant, has the NEXT tile's box in flight while it works on the current one.
+// TMA = the raw RGBA8 source box (tile + halo) arrives by cp.async.bulk.tensor into a landing zone and is decoded
+//       from there; otherwise (FP16/FP32 sources, unaligned pitch) texels are fetched with plain loads.
 constexpr int kEasuRowsPerThread = 5;  // tile rows handled by one warp: ceil(37 / 8)
 constexpr int kEasuColsPerThread = 3;  // 32-wide column blocks: ceil(72 / 32)
 
@@ -372,183 +401,175 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
   uint32_t *sRaw = reinterpret_cast<uint32_t *>(smem_raw + ((tn * 36 + 127) & ~127)); // landing zone (TMA only), 128-byte aligned
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int tilesX = (a.dst.w + kTileW - 1) / kTileW, tilesY = (a.dst.h + kTileH - 1) / kTileH;
-  const int numTiles = tilesX * tilesY;
 
-  auto tile_origin = [&](int t, int &ox0, int &oy0, int &sx0, int &sy0) {
-    const int ty = t / tilesX, tx = t - ty * tilesX;
-    ox0 = tx * kTileW; oy0 = ty * kTileH;
-    // source tile origin: one texel left/above the 'f' texel of the tile's first pixel
-    sx0 = (int)floorf(easu_pos(ox0, a.c0x, a.c0z)) - 1;
-    sy0 = (int)floorf(easu_pos(oy0, a.c0y, a.c0w)) - 1;
-  };
-
-  // Static schedule t = blockIdx.x, += gridDim.x: at radius 2.0 all tiles cost the same.
-  int t = blockIdx.x;
+  // One 64x32 output tile per CTA, handed to the SMs by the hardware block scheduler: a tile costs what its content
+  // asks for (one-colour groups skip the filter, see easu_flat_group), so a static walk over the tiles would leave
+  // the SMs with the most filtered groups finishing last.
+  const int ox0 = blockIdx.x * kTileW, oy0 = blockIdx.y * kTileH;
+  // source tile origin: one texel left/above the 'f' texel of the tile's first pixel
+  const int sx0 = (int)floorf(easu_pos(ox0, a.c0x, a.c0z)) - 1;
+  const int sy0 = (int)floorf(easu_pos(oy0, a.c0y, a.c0w)) - 1;
   if constexpr (TMA) {
     if (tid == 0) {
       mbar_init(&tileBar, 1);
       fence_barrier_init();
-      if (t < numTiles) {
-        int ox0, oy0, sx0, sy0;
-        tile_origin(t, ox0, oy0, sx0, sy0);
-        mbar_arrive_expect_tx(&tileBar, (uint32_t)(rawW * th * 4));
-        tma_load_2d(sRaw, &srcMap, sx0 & ~3, sy0, &tileBar); // box origin 16-byte aligned in x
+      mbar_arrive_expect_tx(&tileBar, (uint32_t)(rawW * th * 4));
+      tma_load_2d(sRaw, &srcMap, sx0 & ~3, sy0, &tileBar); // box origin 16-byte aligned in x
+    }
+    __syncthreads();
+  }
+
+  // float-tile origin and width in source texels: the TMA variant keeps the box's aligned origin
+  const int tx0 = TMA ? (sx0 & ~3) : sx0;
+  const int cols = TMA ? rawW : a.tileW;
+
+  // this warp's 16x16 group and its radius test (warp-uniform)
+  const uint32_t ggx = (uint32_t)(ox0 >> 4) + (warp & 3), ggy = (uint32_t)(oy0 >> 4) + (warp >> 2);
+  const bool inside = group_inside(ggx * 16u + 8u, ggy * 16u + 8u, a.centre, a.radiusSq);
+
+  // ---- stage 1: decode the clamped source tile once, loads batched per thread for ILP -------------
+  if constexpr (TMA) {
+    mbar_wait(&tileBar, 0); // the tile's box has landed (zeros outside the image)
+    const uint32_t *raw = sRaw;
+#pragma unroll
+    for (int i = 0; i < kEasuColsPerThread; ++i) {
+      const int tx = lane + 32 * i;
+      if (tx < cols) {
+        const int rcol = clampi(tx0 + tx, 0, a.src.w - 1) - tx0; // clamp-to-edge: re-read the edge column / row
+        uint32_t px[kEasuRowsPerThread];
+#pragma unroll
+        for (int j = 0; j < kEasuRowsPerThread; ++j) {
+          const int ty = warp + 8 * j;
+          px[j] = ty < th ? raw[(clampi(sy0 + ty, 0, a.src.h - 1) - sy0) * rawW + rcol] : 0u;
+        }
+#pragma unroll
+        for (int j = 0; j < kEasuRowsPerThread; ++j) {
+          const int ty = warp + 8 * j;
+          if (ty < th) {
+            const float4 c = decode_rgb1<FIN>(px[j]);
+            sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y); // luma*2, ffx_fsr1.h:363 (x0.5 exact: FMA-safe)
+            sC[ty * TW + tx] = c;
+          }
+        }
+      }
+    }
+  } else {
+    // plain loads (FP16 / FP32 sources, unaligned pitch): a flat index over the tile, four texels per thread in
+    // flight (no prefetch hides this latency, unlike the TMA variant)
+    const int nTex = cols * th;
+    const uint32_t colsRcp = 0xFFFFFFFFu / (uint32_t)cols + 1u; // ceil(2^32 / cols): q / cols == umulhi(q, colsRcp) for q < 2^32 / cols
+#pragma unroll 4
+    for (int q = tid; q < nTex; q += kThreads) {
+      const int ty = (int)__umulhi((uint32_t)q, colsRcp), tx = q - ty * cols;
+      const int gy = clampi(sy0 + ty, 0, a.src.h - 1), gx = clampi(tx0 + tx, 0, a.src.w - 1);
+      float4 c = get_texel<FIN, ANYIO>(a.src, io.src, gx, gy);
+      sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y);
+      c.w = 1.0f; // EASU ignores source alpha; the fast path accumulates the tap weight through this lane
+      sC[ty * TW + tx] = c;
+    }
+  }
+  // one row term per output row of the tile for the bilinear fallback (skipped when every group is inside)
+  if (tid < kTileH && oy0 + tid < a.dst.h) sRowAxis[tid] = easu_bilinear_axis(oy0 + tid, a.radH, a.src.h, sy0, th);
+  // inside groups whose footprint has one colour store f and need neither the filter nor the features (UNORM
+  // sources only: a float source can hold -0 and NaN, for which the argument at easu_flat_group does not hold)
+  int flatAt = -1;
+  if constexpr (packed32(FIN)) {
+    __syncthreads();
+    if (inside) flatAt = easu_flat_group<TW>(sC, a, lane, (int)ggx * 16, (int)ggy * 16, tx0, sy0);
+  }
+  const int anyFilter = __syncthreads_or(inside && flatAt < 0);
+
+  // ---- stage 2: per-source-texel direction/length features (only where EASU will run) -----------
+  if (anyFilter) {
+#pragma unroll
+    for (int i = 0; i < kEasuColsPerThread; ++i) {
+      const int tx = 1 + lane + 32 * i;
+      if (tx < cols - 1) {
+        float lA[kEasuRowsPerThread], lB[kEasuRowsPerThread], lC[kEasuRowsPerThread], lD[kEasuRowsPerThread],
+            lE[kEasuRowsPerThread];
+#pragma unroll
+        for (int j = 0; j < kEasuRowsPerThread; ++j) {
+          const int ty = 1 + warp + 8 * j;
+          if (ty < th - 1) {
+            const float *l = sL + ty * TW + tx;
+            lA[j] = l[-TW]; lB[j] = l[-1]; lC[j] = l[0]; lD[j] = l[1]; lE[j] = l[TW];
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < kEasuRowsPerThread; ++j) {
+          const int ty = 1 + warp + 8 * j;
+          if (ty < th - 1) sF[ty * TW + tx] = easu_feature(lA[j], lB[j], lC[j], lD[j], lE[j]);
+        }
       }
     }
     __syncthreads();
   }
 
-  uint32_t phase = 0;
-  for (; t < numTiles; t += gridDim.x) {
-    int ox0, oy0, sx0, sy0;
-    tile_origin(t, ox0, oy0, sx0, sy0);
-    // float-tile origin and width in source texels: the TMA variant keeps the box's aligned origin
-    const int tx0 = TMA ? (sx0 & ~3) : sx0;
-    const int cols = TMA ? rawW : a.tileW;
-
-    // this warp's 16x16 group and its radius test (warp-uniform)
-    const uint32_t ggx = (uint32_t)(ox0 >> 4) + (warp & 3), ggy = (uint32_t)(oy0 >> 4) + (warp >> 2);
-    const bool inside = group_inside(ggx * 16u + 8u, ggy * 16u + 8u, a.centre, a.radiusSq);
-
-    // ---- stage 1: decode the clamped source tile once, loads batched per thread for ILP -------------
-    if constexpr (TMA) {
-      mbar_wait(&tileBar, phase); // this tile's box has landed (zeros outside the image)
-      phase ^= 1u;
-      const uint32_t *raw = sRaw;
-#pragma unroll
-      for (int i = 0; i < kEasuColsPerThread; ++i) {
-        const int tx = lane + 32 * i;
-        if (tx < cols) {
-          const int rcol = clampi(tx0 + tx, 0, a.src.w - 1) - tx0; // clamp-to-edge: re-read the edge column / row
-          uint32_t px[kEasuRowsPerThread];
-#pragma unroll
-          for (int j = 0; j < kEasuRowsPerThread; ++j) {
-            const int ty = warp + 8 * j;
-            px[j] = ty < th ? raw[(clampi(sy0 + ty, 0, a.src.h - 1) - sy0) * rawW + rcol] : 0u;
-          }
-#pragma unroll
-          for (int j = 0; j < kEasuRowsPerThread; ++j) {
-            const int ty = warp + 8 * j;
-            if (ty < th) {
-              const float4 c = decode_rgb1<FIN>(px[j]);
-              sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y); // luma*2, ffx_fsr1.h:363 (x0.5 exact: FMA-safe)
-              sC[ty * TW + tx] = c;
-            }
-          }
+  // ---- stage 3: one warp per 16x16 group, 8 pixels per lane --------------------------------------
+  const int x = (int)ggx * 16 + (lane & 15);
+  if (x < a.dst.w) {
+    const int yFirst = (int)ggy * 16 + (lane >> 4);
+    if (inside && flatAt >= 0) {
+      const float4 f = sC[flatAt];
+      if constexpr (ANYIO) {
+        for (int y = yFirst; y < a.dst.h && y < yFirst + 16; y += 2) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, f.x, f.y, f.z);
+      } else {
+        const texel_t<FOUT> v = encode_opaque<FOUT>(f.x, f.y, f.z);
+        uint8_t *out = a.dst.ptr + (size_t)yFirst * a.dst.pitch + (size_t)x * sizeof(texel_t<FOUT>);
+        for (int y = yFirst; y < a.dst.h && y < yFirst + 16; y += 2) {
+          *reinterpret_cast<texel_t<FOUT> *>(out) = v;
+          out += 2 * (size_t)a.dst.pitch;
+        }
+      }
+    } else if (inside) {
+      const float ppx_full = easu_pos(x, a.c0x, a.c0z);
+      const float fpx = floorf(ppx_full);
+      const float ppx = ppx_full - fpx;
+      const int ix = (int)fpx - tx0 - sy0 * TW; // tile offset of texel (fpx, 0)
+      const int yEnd = min(yFirst + 16, a.dst.h);
+      // pitched target: the store address advances by two rows per pixel instead of being formed from (x, y)
+      uint8_t *out = a.dst.ptr + (size_t)yFirst * a.dst.pitch + (size_t)x * sizeof(texel_t<FOUT>);
+#pragma unroll 2
+      for (int y = yFirst; y < yEnd; y += 2) {
+        const float ppy_full = easu_pos(y, a.c0y, a.c0w);
+        const float fpy = floorf(ppy_full);
+        const int o = (int)fpy * TW + ix;
+        float3 c;
+        if constexpr (kStrict) c = easu_filter<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
+        else c = easu_filter_fast<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
+        if constexpr (ANYIO) {
+          put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
+        } else {
+          *reinterpret_cast<texel_t<FOUT> *>(out) = encode_opaque<FOUT>(c.x, c.y, c.z);
+          out += 2 * (size_t)a.dst.pitch;
         }
       }
     } else {
-      // plain loads (FP16 / FP32 sources, unaligned pitch): a flat index over the tile, four texels per thread in
-      // flight (no prefetch hides this latency, unlike the TMA variant)
-      const int nTex = cols * th;
-      const uint32_t colsRcp = 0xFFFFFFFFu / (uint32_t)cols + 1u; // ceil(2^32 / cols): q / cols == umulhi(q, colsRcp) for q < 2^32 / cols
-#pragma unroll 4
-      for (int q = tid; q < nTex; q += kThreads) {
-        const int ty = (int)__umulhi((uint32_t)q, colsRcp), tx = q - ty * cols;
-        const int gy = clampi(sy0 + ty, 0, a.src.h - 1), gx = clampi(tx0 + tx, 0, a.src.w - 1);
-        float4 c = get_texel<FIN, ANYIO>(a.src, io.src, gx, gy);
-        sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y);
-        c.w = 1.0f; // EASU ignores source alpha; the fast path accumulates the tap weight through this lane
-        sC[ty * TW + tx] = c;
-      }
-    }
-    // one row term per output row of the tile for the bilinear fallback (skipped when every group is inside)
-    if (tid < kTileH && oy0 + tid < a.dst.h) sRowAxis[tid] = easu_bilinear_axis(oy0 + tid, a.radH, a.src.h, sy0, th);
-    const int anyInside = __syncthreads_or(inside);
-    const int tn2 = t + gridDim.x;
-    if constexpr (TMA) {
-      // the landing zone is fully decoded: refill it with the NEXT tile's box while this tile is filtered
-      if (tid == 0 && tn2 < numTiles) {
-        int nox, noy, nsx, nsy;
-        tile_origin(tn2, nox, noy, nsx, nsy);
-        fence_proxy_async();
-        mbar_arrive_expect_tx(&tileBar, (uint32_t)(rawW * th * 4));
-        tma_load_2d(sRaw, &srcMap, nsx & ~3, nsy, &tileBar);
-      }
-    }
-
-    // ---- stage 2: per-source-texel direction/length features (only where EASU will run) -----------
-    if (anyInside) {
-#pragma unroll
-      for (int i = 0; i < kEasuColsPerThread; ++i) {
-        const int tx = 1 + lane + 32 * i;
-        if (tx < cols - 1) {
-          float lA[kEasuRowsPerThread], lB[kEasuRowsPerThread], lC[kEasuRowsPerThread], lD[kEasuRowsPerThread],
-              lE[kEasuRowsPerThread];
-#pragma unroll
-          for (int j = 0; j < kEasuRowsPerThread; ++j) {
-            const int ty = 1 + warp + 8 * j;
-            if (ty < th - 1) {
-              const float *l = sL + ty * TW + tx;
-              lA[j] = l[-TW]; lB[j] = l[-1]; lC[j] = l[0]; lD[j] = l[1]; lE[j] = l[TW];
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < kEasuRowsPerThread; ++j) {
-            const int ty = 1 + warp + 8 * j;
-            if (ty < th - 1) sF[ty * TW + tx] = easu_feature(lA[j], lB[j], lC[j], lD[j], lE[j]);
-          }
-        }
-      }
-      __syncthreads();
-    }
-
-    // ---- stage 3: one warp per 16x16 group, 8 pixels per lane --------------------------------------
-    const int x = (int)ggx * 16 + (lane & 15);
-    if (x < a.dst.w) {
-      const int yFirst = (int)ggy * 16 + (lane >> 4);
-      if (inside) {
-        const float ppx_full = easu_pos(x, a.c0x, a.c0z);
-        const float fpx = floorf(ppx_full);
-        const float ppx = ppx_full - fpx;
-        const int ix = (int)fpx - tx0 - sy0 * TW; // tile offset of texel (fpx, 0)
-        const int yEnd = min(yFirst + 16, a.dst.h);
-        // pitched target: the store address advances by two rows per pixel instead of being formed from (x, y)
-        uint8_t *out = a.dst.ptr + (size_t)yFirst * a.dst.pitch + (size_t)x * sizeof(texel_t<FOUT>);
+      const BilinAxis ax = easu_bilinear_axis(x, a.radW, a.src.w, tx0, cols);
+      constexpr bool direct = PAIRED && (FOUT == OVRFSR_FORMAT_RGBA8 || FOUT == OVRFSR_FORMAT_RGB10A2);
+      // the intermediate is still needed where RCAS of an edge-adjacent inside group reads across the group edge
+      const bool mid = !direct || group_inside(ggx * 16u - 8u, ggy * 16u + 8u, a.centre, a.radiusSq) ||
+                       group_inside(ggx * 16u + 24u, ggy * 16u + 8u, a.centre, a.radiusSq) ||
+                       group_inside(ggx * 16u + 8u, ggy * 16u - 8u, a.centre, a.radiusSq) ||
+                       group_inside(ggx * 16u + 8u, ggy * 16u + 24u, a.centre, a.radiusSq);
 #pragma unroll 2
-        for (int y = yFirst; y < yEnd; y += 2) {
-          const float ppy_full = easu_pos(y, a.c0y, a.c0w);
-          const float fpy = floorf(ppy_full);
-          const int o = (int)fpy * TW + ix;
-          float3 c;
-          if constexpr (kStrict) c = easu_filter<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
-          else c = easu_filter_fast<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
-          if constexpr (ANYIO) {
-            put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
+      for (int k = 0; k < 8; ++k) {
+        const int y = yFirst + 2 * k;
+        if (y >= a.dst.h) break;
+        const float3 c = easu_bilinear(sC, TW, ax, sRowAxis[y - oy0]);
+        if (mid) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
+        if constexpr (direct) {
+          if (a.tintGB == 1.0f) {
+            // RCAS's copy is the identity on UNORM codes (decode -> x1 -> encode): the same bits go to the final image
+            put_opaque<FOUT, ANYIO>(a.direct, io.direct, x, y, c.x, c.y, c.z);
           } else {
-            *reinterpret_cast<texel_t<FOUT> *>(out) = encode_opaque<FOUT>(c.x, c.y, c.z);
-            out += 2 * (size_t)a.dst.pitch;
-          }
-        }
-      } else {
-        const BilinAxis ax = easu_bilinear_axis(x, a.radW, a.src.w, tx0, cols);
-        constexpr bool direct = PAIRED && (FOUT == OVRFSR_FORMAT_RGBA8 || FOUT == OVRFSR_FORMAT_RGB10A2);
-        // the intermediate is still needed where RCAS of an edge-adjacent inside group reads across the group edge
-        const bool mid = !direct || group_inside(ggx * 16u - 8u, ggy * 16u + 8u, a.centre, a.radiusSq) ||
-                         group_inside(ggx * 16u + 24u, ggy * 16u + 8u, a.centre, a.radiusSq) ||
-                         group_inside(ggx * 16u + 8u, ggy * 16u - 8u, a.centre, a.radiusSq) ||
-                         group_inside(ggx * 16u + 8u, ggy * 16u + 24u, a.centre, a.radiusSq);
-#pragma unroll 2
-        for (int k = 0; k < 8; ++k) {
-          const int y = yFirst + 2 * k;
-          if (y >= a.dst.h) break;
-          const float3 c = easu_bilinear(sC, TW, ax, sRowAxis[y - oy0]);
-          if (mid) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
-          if constexpr (direct) {
-            if (a.tintGB == 1.0f) {
-              // RCAS's copy is the identity on UNORM codes (decode -> x1 -> encode): the same bits go to the final image
-              put_opaque<FOUT, ANYIO>(a.direct, io.direct, x, y, c.x, c.y, c.z);
-            } else {
-              // OutputTexture[p] = mul * InputTexture[p] on the stored-then-loaded value (fsr_rcas.hlsl:45-53)
-              const float4 m = mid_roundtrip<FOUT>(c.x, c.y, c.z);
-              put_texel<FOUT, ANYIO>(a.direct, io.direct, x, y, 1.0f * m.x, a.tintGB * m.y, a.tintGB * m.z, 1.0f * m.w);
-            }
+            // OutputTexture[p] = mul * InputTexture[p] on the stored-then-loaded value (fsr_rcas.hlsl:45-53)
+            const float4 m = mid_roundtrip<FOUT>(c.x, c.y, c.z);
+            put_texel<FOUT, ANYIO>(a.direct, io.direct, x, y, 1.0f * m.x, a.tintGB * m.y, a.tintGB * m.z, 1.0f * m.w);
           }
         }
       }
     }
-    __syncthreads(); // every warp is done with this tile before the next decode overwrites it
   }
 }
 

@@ -48,7 +48,7 @@ def loops(ins):
 def per_pixel(so):
     k = kernels(so)
     e, r = [s for _, s in k["easu"]], [s for _, s in k["rcas"]]
-    # EASU: the innermost large loop is stage 3's filter loop; the outer ones are the persistent tile loop
+    # EASU: the innermost large loop is stage 3's filter loop
     el = [(a, b) for a, b in loops(k["easu"]) if b - a + 1 >= 500]
     fa, fb = min(el, key=lambda ab: ab[1] - ab[0])
     # RCAS: the decode loop is its only loop with an STS
