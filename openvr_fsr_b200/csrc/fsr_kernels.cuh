@@ -471,7 +471,9 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
   // one row term per output row of the tile for the bilinear fallback (skipped when every group is inside)
   if (tid < kTileH && oy0 + tid < a.dst.h) sRowAxis[tid] = easu_bilinear_axis(oy0 + tid, a.radH, a.src.h, sy0, th);
   // inside groups whose footprint has one colour store f and need neither the filter nor the features (UNORM
-  // sources only: a float source can hold -0 and NaN, for which the argument at easu_flat_group does not hold)
+  // sources only: a float source can hold -0 and NaN, for which the argument at easu_flat_group does not hold).
+  // The skip is decided here, per group, never at launch: which kernel a dispatch launches depends on formats and
+  // layouts only, not on texel values (tests/test_gpu_float_signed.py relies on that for its coverage count).
   int flatAt = -1;
   if constexpr (packed32(FIN)) {
     __syncthreads();

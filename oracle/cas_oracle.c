@@ -17,8 +17,8 @@
 #include "ovr_oracle.h"
 #include "ovr_glue.h"
 
-static inline float mn2(float a, float b) { return fminf(a, b); }
-static inline float mx2(float a, float b) { return fmaxf(a, b); }
+static inline float mn2(float a, float b) { return ovo_min(a, b); }
+static inline float mx2(float a, float b) { return ovo_max(a, b); }
 static inline float mn3(float x, float y, float z) { return mn2(x, mn2(y, z)); } /* AMin3F1 */
 static inline float mx3(float x, float y, float z) { return mx2(x, mx2(y, z)); } /* AMax3F1 */
 static inline float prx_lo_rcp(float a) { return ovo_u2f(0x7ef07ebbu - ovo_f2u(a)); }

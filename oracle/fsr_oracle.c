@@ -101,6 +101,10 @@ int ovo_group_inside(uint32_t gx, uint32_t gy, uint32_t gw, uint32_t gh, const u
   return ovo_group_inside_(gx, gy, gw, gh, centre, radiusSq);
 }
 
+float ovo_hlsl_min(float a, float b) { return ovo_min(a, b); }
+float ovo_hlsl_max(float a, float b) { return ovo_max(a, b); }
+float ovo_hlsl_saturate(float a) { return ovo_sat(a); }
+
 /* ------------------------------------------------------------------------
  * approximations, ffx_a.h:1843-1845 (integer bit tricks, portable bit-exactly)
  * ---------------------------------------------------------------------- */

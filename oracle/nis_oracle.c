@@ -31,14 +31,14 @@ const float *ovo_nis_coef_usm(void) { coef_init(); return &g_usm[0][0]; }
 /* NVScalerUpdateConfig, NIS_Config.h:144-241 (SDR branch), argument pattern of PostProcessor.cpp:308/433 */
 static int nis_update(ovo_nis_config *c, float sharpness, uint32_t inW, uint32_t inH, uint32_t outW, uint32_t outH) {
   memset(c, 0, sizeof(*c));
-  sharpness = fmaxf(fminf(1.f, sharpness), 0.f);
+  sharpness = ovo_max(ovo_min(1.f, sharpness), 0.f);
   const float slider = sharpness - 0.5f;
   const float MinScale = (slider >= 0.0f) ? 1.25f : 1.0f;
   const float LimitScale = (slider >= 0.0f) ? 1.25f : 1.0f;
   const float kMinContrastRatio = 2.0f, kMaxContrastRatio = 10.0f, kSharpStartY = 0.45f, kSharpEndY = 0.9f;
-  const float kSharpStrengthMin = fmaxf(0.0f, 0.4f + slider * MinScale * 1.2f);
+  const float kSharpStrengthMin = ovo_max(0.0f, 0.4f + slider * MinScale * 1.2f);
   const float kSharpStrengthMax = 1.6f + slider * 1.8f;
-  const float kSharpLimitMin = fmaxf(0.1f, 0.14f + slider * LimitScale * 0.32f);
+  const float kSharpLimitMin = ovo_max(0.1f, 0.14f + slider * LimitScale * 0.32f);
   const float kSharpLimitMax = 0.5f + slider * LimitScale * 0.6f;
   c->kInputViewportWidth = inW; c->kInputViewportHeight = inH;
   c->kOutputViewportWidth = outW; c->kOutputViewportHeight = outH;

@@ -27,10 +27,24 @@
 static inline float ovo_u2f(uint32_t u) { float f; memcpy(&f, &u, 4); return f; }
 static inline uint32_t ovo_f2u(float f) { uint32_t u; memcpy(&u, &f, 4); return u; }
 
-/* NaN-ignoring min/max and saturate(NaN)=0: HLSL min/max/saturate semantics */
-static inline float ovo_min(float a, float b) { return fminf(a, b); }
-static inline float ovo_max(float a, float b) { return fmaxf(a, b); }
-static inline float ovo_sat(float a) { return fminf(1.0f, fmaxf(0.0f, a)); }
+/* HLSL min / max / saturate.  D3D11 pins NaN handling (the other operand; saturate(NaN) = 0) and leaves the sign of
+ * min(+0, -0) to the implementation; C's fminf / fmaxf leave it open too (glibc returns the first operand).  The checker
+ * pins the rule sm_90a's FMNMX follows, which tests/test_gpu_minmax_rule.py measures on the device: IEEE 754-2019
+ * minimumNumber / maximumNumber -- NaN ignored, -0 < +0, independent of operand order.  No libm call: the bits must
+ * not depend on the host's C library.  saturate(x) = min(1, max(+0, x)), so saturate(-0) = +0 (FADD.SAT: +0 + -0). */
+static inline float ovo_min(float a, float b) {
+  if (a != a) return b;
+  if (b != b) return a;
+  if (a != b) return a < b ? a : b;
+  return (ovo_f2u(a) & 0x80000000u) ? a : b; /* equal: only a zero pair can differ in bits; -0 wins */
+}
+static inline float ovo_max(float a, float b) {
+  if (a != a) return b;
+  if (b != b) return a;
+  if (a != b) return a > b ? a : b;
+  return (ovo_f2u(a) & 0x80000000u) ? b : a; /* equal: +0 wins */
+}
+static inline float ovo_sat(float a) { return ovo_min(1.0f, ovo_max(0.0f, a)); }
 
 /* IEEE half <-> float (exact up-conversion, round-to-nearest-even down-conversion) */
 static inline float ovo_half_to_float(uint16_t h) {

@@ -71,8 +71,8 @@ def build(force: bool = False) -> None:
     ref_root = Path(os.environ.get("OVRFSR_REFERENCE", "/root/reference"))
     ref_so = HERE / "_ref" / "libovrfsr_ref.so"
     if (ref_root / "src/fsr/ffx_fsr1.h").exists():
-        shim = list((HERE / "ref_shim").glob("*.cpp")) + [HERE / "build_ref.sh", HERE / "ovr_glue.h",
-                                                           HERE / "fsr_entry.inc"]
+        shim = [p for p in (HERE / "ref_shim").iterdir() if p.suffix in (".cpp", ".h", ".inc")] + \
+            [HERE / "build_ref.sh", HERE / "ovr_glue.h", HERE / "ovr_oracle.h"] + list(HERE.glob("*_entry.inc"))
         if force or not ref_so.exists() or any(p.stat().st_mtime > ref_so.stat().st_mtime for p in shim if p.exists()):
             subprocess.check_call(["bash", str(HERE / "build_ref.sh")], stdout=subprocess.DEVNULL)
 
@@ -116,6 +116,9 @@ def oracle_lib():
             lib.ovo_nis_coef_usm.restype = f32p
         lib.ovo_group_inside.argtypes = [C.c_uint32] * 4 + [u32p, C.c_uint32]
         lib.ovo_group_inside.restype = C.c_int
+        for name, n in (("ovo_hlsl_min", 2), ("ovo_hlsl_max", 2), ("ovo_hlsl_saturate", 1)):
+            getattr(lib, name).argtypes = [C.c_float] * n
+            getattr(lib, name).restype = C.c_float
         lib.ovo_cas_setup.argtypes = [C.POINTER(CasConstants)] + [C.c_float] * 6
         lib.ovo_cas.argtypes = [_PI, _PI, C.POINTER(CasConstants), C.c_int, C.c_int]
         lib.ovo_cas.restype = C.c_int

@@ -60,18 +60,19 @@ static inline AF3 &operator+=(AF3 &a, AF3 b) { a.x += b.x; a.y += b.y; a.z += b.
 static inline AF4 operator*(AF4 a, AF4 b) { return AF4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w); }
 static inline AF4 operator+(AF4 a, AF4 b) { return AF4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
 static inline ASU2 operator+(ASU2 a, ASU2 b) { return ASU2(a.x + b.x, a.y + b.y); }
-static inline float min(float a, float b) { return fminf(a, b); }
-static inline float max(float a, float b) { return fmaxf(a, b); }
+// min / max / saturate are the checker's pinned rule (ovr_glue.h ovo_min / ovo_max / ovo_sat), not libm's
+static inline float min(float a, float b) { return ovo_min(a, b); }
+static inline float max(float a, float b) { return ovo_max(a, b); }
 static inline float abs(float a) { return fabsf(a); }
-static inline float clamp(float x, float lo, float hi) { return fminf(fmaxf(x, lo), hi); }
+static inline float clamp(float x, float lo, float hi) { return ovo_min(ovo_max(x, lo), hi); }
 static inline AF2 floor(AF2 a) { return AF2(floorf(a.x), floorf(a.y)); }
-static inline AF3 min(AF3 a, AF3 b) { return AF3(fminf(a.x, b.x), fminf(a.y, b.y), fminf(a.z, b.z)); }
-static inline AF3 max(AF3 a, AF3 b) { return AF3(fmaxf(a.x, b.x), fmaxf(a.y, b.y), fmaxf(a.z, b.z)); }
+static inline AF3 min(AF3 a, AF3 b) { return AF3(ovo_min(a.x, b.x), ovo_min(a.y, b.y), ovo_min(a.z, b.z)); }
+static inline AF3 max(AF3 a, AF3 b) { return AF3(ovo_max(a.x, b.x), ovo_max(a.y, b.y), ovo_max(a.z, b.z)); }
 // ffx_a.h:1141,1143,1166,1168,1196,1206 (A_HLSL definitions; one-line wrappers around the intrinsics)
 static inline AF1 AMax3F1(AF1 x, AF1 y, AF1 z) { return max(x, max(y, z)); }
 static inline AF1 AMin3F1(AF1 x, AF1 y, AF1 z) { return min(x, min(y, z)); }
 static inline AF3 AMax3F3(AF3 x, AF3 y, AF3 z) { return max(x, max(y, z)); }
 static inline AF3 AMin3F3(AF3 x, AF3 y, AF3 z) { return min(x, min(y, z)); }
 static inline AF1 ARcpF1(AF1 x) { return 1.0f / x; }                 // rcp(x)
-static inline AF1 ASatF1(AF1 x) { return fminf(1.0f, fmaxf(0.0f, x)); } // saturate(x)
+static inline AF1 ASatF1(AF1 x) { return ovo_sat(x); }               // saturate(x)
 

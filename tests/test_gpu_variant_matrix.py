@@ -150,8 +150,9 @@ def _seed(key):
     return 1 + sum((i + 3) * a for i, a in enumerate(key[2])) + len(key[1])
 
 
-def _stateless(key):
-    """EASU / RCAS / NVScaler / NVSharpen / CAS / fused: one ovrfsr_dispatch_* call per I/O layout"""
+def _stateless(key, content=None):
+    """EASU / RCAS / NVScaler / NVSharpen / CAS / fused: one ovrfsr_dispatch_* call per I/O layout.  content(fmt, w, h,
+    seed) -> source array (default: _content)"""
     import openvr_fsr_b200 as ovr
     from oracle import pyoracle as po
     mode, kernel, args = key
@@ -210,7 +211,7 @@ def _stateless(key):
         raise AssertionError(key)
 
     def run(dev):
-        src = _content(sfmt, W, H, _seed(key))
+        src = (content or _content)(sfmt, W, H, _seed(key))
         want = oracle(src, _tag(fout))
         out = []
         for where, kinds in layouts:
@@ -222,7 +223,7 @@ def _stateless(key):
     return Case(kernel, mode, {key}, run, kl.describe(key))
 
 
-def _paired(mode, fin, tw, tma, anyio):
+def _paired(mode, fin, tw, tma, anyio, content=None):
     """the context path with a UNORM output: paired EASU + RCAS, both eyes (apply_pair / apply_pair_into)"""
     import torch
     import openvr_fsr_b200 as ovr
@@ -235,7 +236,7 @@ def _paired(mode, fin, tw, tma, anyio):
 
     def run(dev):
         ow, oh = ovr.output_size(W, H, scale)
-        eyes = [_content(fin, W, H, 40 + fin + 2 * e) for e in (0, 1)]
+        eyes = [(content or _content)(fin, W, H, 40 + fin + 2 * e) for e in (0, 1)]
         pp = ovr.PostProcessor(ovr.Config(fsrEnabled=True, renderScale=scale, sharpness=SHARP, radius=RADIUS, projCentre=PROJ,
                                           debugMode=debug, mathMode=_mathmode(mode)))
         if anyio and layered:
@@ -314,7 +315,7 @@ def _host_entry():
     return Case("host entry", "strict", keys, run, "strict:apply_host (tight host rows)")
 
 
-def _rgb32f_source():
+def _rgb32f_source(content=None):
     """an R32G32B32_FLOAT eye: expanded to RGBA32F (alpha 1), then the paired passes"""
     import torch
     import openvr_fsr_b200 as ovr
@@ -324,7 +325,7 @@ def _rgb32f_source():
 
     def run(dev):
         ow, oh = ovr.output_size(W, H, 0.75)
-        rgba = _content(kl.RGBA32F, W, H, 9)
+        rgba = (content or _content)(kl.RGBA32F, W, H, 9)
         rgb = np.ascontiguousarray(rgba[..., :3])
         pp = ovr.PostProcessor(ovr.Config(fsrEnabled=True, renderScale=0.75, sharpness=SHARP, radius=RADIUS, projCentre=PROJ))
         got = pp.apply(0, torch.from_numpy(rgb).to(dev), fmt=RGB32F).cpu().numpy()
@@ -335,22 +336,23 @@ def _rgb32f_source():
     return Case("rgb32f source", "strict", keys, run, "strict:apply (R32G32B32_FLOAT source)")
 
 
-def case_for(key):
+def case_for(key, content=None):
+    """the case that launches `key`; content(fmt, w, h, seed) replaces the sources of the FSR / NIS / CAS drivers"""
     mode, kernel, args = key
     p = dict(zip(kl.PARAMS[kernel], args))
     if kernel == "easu_kernel" and p["PAIRED"]:
-        return _paired(mode, p["FIN"], p["TW"], p["TMA"], p["ANYIO"])
+        return _paired(mode, p["FIN"], p["TW"], p["TMA"], p["ANYIO"], content)
     if kernel == "rcas_kernel" and p["PAIRED"]:
-        return _paired(mode, p["FIN"], 60, 1, p["ANYIO"])
+        return _paired(mode, p["FIN"], 60, 1, p["ANYIO"], content)
     if kernel in ("easu_kernel", "rcas_kernel", "nis_scaler_kernel", "nis_sharpen_kernel", "cas_sharpen_kernel",
                   "cas_scale_kernel", "fsr_fused_kernel"):
-        return _stateless(key)
+        return _stateless(key, content)
     if kernel == "resolve_msaa_kernel":
         return _resolve(key)
     if kernel == "repitch_rows_kernel":
         return _host_entry()
     if kernel == "expand_rgb32f_kernel":
-        return _rgb32f_source()
+        return _rgb32f_source(content)
     return None
 
 
