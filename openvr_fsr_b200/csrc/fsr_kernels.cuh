@@ -650,6 +650,28 @@ __device__ __forceinline__ float3 rcas_filter_mode(const float4 b, const float4 
   else return rcas_filter_fast(b, d, e, f, h, sharp);
 }
 
+// One-colour groups.  FsrRcasF reads the five texels b / d / e / f / h of a pixel's cross and nothing else (alpha
+// included: it ignores it), so where every texel any cross of a group reads has the same RGB bits, every pixel of the
+// group gets the same value, the filter of its first pixel.  Bit equality, not float equality: it holds for -0, NaN
+// and HDR texels, in both math modes, with no lemma on the filter.  The union of the crosses is the group plus a
+// 1-texel ring; this tests the whole 18 x 18 tile window w (corners included, which is conservative).  A partial group
+// at the right / bottom image edge reads its ring from the zeros outside the image (Texture2D.Load), and every window
+// texel past the edge is such a zero, so testing the whole window gives the answer the in-image part would.
+// Called by all 32 lanes of a warp: two window rows per step (half-warps at columns 0-15 and 2-17), leaving at the
+// first step that finds a second colour.
+__device__ __forceinline__ bool rcas_flat_group(const float4 *__restrict__ w, int lane) {
+  const float4 ref = w[kRcasTW + 1];
+  const float4 *t = w + (lane & 15) + 2 * (lane >> 4);
+  uint32_t diff = 0;
+#pragma unroll 1
+  for (int r = 0; diff == 0 && r < 18 * kRcasTW; r += 2 * kRcasTW) {
+    const float4 u = t[r], v = t[r + kRcasTW];
+    diff = __reduce_or_sync(0xFFFFFFFFu, (f2u(u.x) ^ f2u(ref.x)) | (f2u(u.y) ^ f2u(ref.y)) | (f2u(u.z) ^ f2u(ref.z)) |
+                                             (f2u(v.x) ^ f2u(ref.x)) | (f2u(v.y) ^ f2u(ref.y)) | (f2u(v.z) ^ f2u(ref.z)));
+  }
+  return diff == 0;
+}
+
 // four adjacent output texels -> memory; one 128-bit store when the format is 4 bytes wide and alignment allows
 template <int FOUT>
 __device__ __forceinline__ void store_quad(const ImageRW &dst, bool vec, int x, int y, const float4 (&px)[4]) {
@@ -754,6 +776,12 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
     }
   }
   __syncthreads();
+  // inside groups whose crosses read one RGB store their first pixel's value (rcas_flat_group).  The skip is decided
+  // here, per group, never at launch: which kernel a dispatch launches depends on formats and layouts only, not on
+  // texel values (tests/test_gpu_float_signed.py relies on that for its coverage count).  Tested before the lanes
+  // past the image edge leave, as the vote needs the whole warp, and by outside groups too: behind the radius test
+  // ptxas keeps the store descriptor in vector registers and converts it before every store of the column.
+  const bool flat = rcas_flat_group(sC + (warp >> 2) * 16 * kRcasTW + (warp & 3) * 16, lane) && inside;
 
   const int x = (int)ggx * 16 + (lane & 15);
   if (x >= a.dst.w) return;
@@ -761,14 +789,32 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
   const float4 *p = sC + (y0 - sy0) * kRcasTW + (x - sx0);
   if (inside) {
     float4 b = p[-kRcasTW], e = p[0];
+    // pitched target: the store address advances by one row per pixel instead of being formed from (x, y)
+    uint8_t *out = a.dst.ptr + (size_t)y0 * a.dst.pitch + (size_t)x * sizeof(texel_t<FOUT>);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const int y = y0 + k;
       if (y >= a.dst.h) break;
       const float4 h = p[kRcasTW], d = p[-1], f = p[1];
       const float3 c = rcas_filter_mode<FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_BGRA8>(b, d, e, f, h, a.sharp);
-      put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
-      b = e; e = h; p += kRcasTW;
+      if constexpr (ANYIO) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
+      else *reinterpret_cast<texel_t<FOUT> *>(out) = encode_opaque<FOUT>(c.x, c.y, c.z);
+      if (k == 0 && flat) {
+        // the other rows of a one-colour group take row 0's value
+        const int yEnd = min(y0 + 8, a.dst.h);
+        if constexpr (ANYIO) {
+          for (int yy = y0 + 1; yy < yEnd; ++yy) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, yy, c.x, c.y, c.z);
+        } else {
+          const texel_t<FOUT> v = encode_opaque<FOUT>(c.x, c.y, c.z);
+#pragma unroll 1
+          for (int yy = y0 + 1; yy < yEnd; ++yy) {
+            out += a.dst.pitch;
+            *reinterpret_cast<texel_t<FOUT> *>(out) = v;
+          }
+        }
+        return;
+      }
+      b = e; e = h; p += kRcasTW; out += a.dst.pitch;
     }
   } else if constexpr (!PAIRED) {
     // OutputTexture[p] = mul * InputTexture[p], alpha included (fsr_rcas.hlsl:45-53)
