@@ -198,6 +198,23 @@ OVRFSR_API int ovrfsr_apply_into(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *s
 OVRFSR_API int ovrfsr_apply_pair_into(ovrfsr_ctx *ctx, const ovrfsr_image *src_left, const ovrfsr_image *src_right,
                                       int only_one_eye, const ovrfsr_image dst[2], void *stream);
 
+/* ---- foveation: the radius mask follows the gaze ------------------------------------------
+ * Focus of the radius mask for `eye`, in the same normalised coordinates as ovrfsr_config::proj_centre
+ * (x right, y down, [0,1]; relative to the eye's half for a side-by-side texture).  Takes the place of that
+ * eye's projection centre in the imageCentre words; the radius is unchanged.  No reset, no reallocation.
+ * May be called from any thread, concurrently with the ctx's apply calls.  OVRFSR_ERR_INVALID for
+ * eye not in {0,1} or x/y not finite or outside [0,1].
+ * Late-latched: while some eye has a focus, each apply (every ovrfsr_apply* entry) starts with a 16-byte
+ * host->device copy of its eye's centre words on its stream, and the masked kernels read them from device
+ * memory, so a frame uses the focus set before that copy RUNS; a captured CUDA graph follows later calls on
+ * every replay.  Each (x, y) pair is published with one 64-bit store: a copy that overlaps an update may mix
+ * the two centre pairs of a block, never the x of one update with the y of another.  The focus survives
+ * ovrfsr_reset, ovrfsr_set_config and source-size changes.  Host memory only: no CUDA call, no device needed. */
+OVRFSR_API int ovrfsr_set_focus(ovrfsr_ctx *ctx, int eye, float x, float y);
+/* Back to the projection centre for `eye` (the reference's behaviour).  Graphs captured with a focus read the
+ * projection centre from then on; once no eye has a focus, applies stop issuing the copy. */
+OVRFSR_API int ovrfsr_clear_focus(ovrfsr_ctx *ctx, int eye);
+
 /* ---- individual dispatches (ApplyUpscaling / ApplySharpening, PostProcessor.cpp:385-401,483-496) --
  * Stateless: explicit constant blocks, caller-owned destination.  math_mode as ovrfsr_math. */
 /* g_FSRUpscaleShader: consts = UpscaleConstants, 24 x u32 (PostProcessor.cpp:276-283) */

@@ -205,6 +205,16 @@ class PostProcessor:
         self.config = config
         L.check(L.lib().ovrfsr_set_config(self._ctx, C.byref(config.to_c())), "ovrfsr_set_config", self._ctx)
 
+    def set_focus(self, eye: int, x: float, y: float):
+        """ovrfsr_set_focus: centre `eye`'s radius mask on (x, y) -- normalised like Config.projCentre, x right, y down,
+        in [0, 1] -- instead of its projection centre.  Host memory only (any thread, no device needed); every apply whose
+        GPU work starts afterwards uses it, a captured CUDA graph on its next replay."""
+        L.check(L.lib().ovrfsr_set_focus(self._ctx, eye, x, y), "ovrfsr_set_focus", self._ctx)
+
+    def clear_focus(self, eye: int):
+        """ovrfsr_clear_focus: back to the projection centre for `eye`."""
+        L.check(L.lib().ovrfsr_clear_focus(self._ctx, eye), "ovrfsr_clear_focus", self._ctx)
+
     def apply(self, eye: int, texture, bounds: TextureBounds | None = None, fmt: int | None = None, stream=None,
               samples: int = 1):
         """vr::PostProcessor::Apply.  Returns a torch tensor VIEW of the ctx-owned output (valid until the next

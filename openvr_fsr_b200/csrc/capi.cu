@@ -6,6 +6,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <mutex>
 #include <new>
 #include <ctime>
 #include <string>
@@ -99,6 +100,21 @@ cudaError_t expand_rgb32f(const ovrfsr_image &src, const ovrfsr_image &dst, cuda
   return cudaGetLastError();
 }
 
+// The radius mask's focus (ovrfsr_set_focus).  `slot` (pinned host memory, one 16-byte block of imageCentre words per
+// eye) is what each apply's H2D copy reads when it runs on the GPU; it is written under `mu` only, each (x, y) pair
+// with one aligned 64-bit store, so a copy that overlaps an update sees whole pairs.  No CUDA call is made under `mu`.
+struct Focus {
+  std::mutex mu;
+  bool set[2] = {false, false};
+  float xy[2][2] = {};
+  // what the words are computed for: the ctx's config, layout and output size at its last prepare_resources
+  bool ready = false;
+  ovrfsr_config cfg{};
+  bool onlyOneEye = true;
+  uint32_t outW = 0, outH = 0;
+  uint32_t *slot = nullptr; // [2][4], allocated by the first apply that needs it
+};
+
 } // namespace
 
 struct ovrfsr_ctx {
@@ -137,6 +153,11 @@ struct ovrfsr_ctx {
   // ovrfsr_apply_pair: the right eye's chain runs on this stream between a fork and a join event
   cudaStream_t pairStream = nullptr;
   cudaEvent_t pairFork = nullptr, pairJoin = nullptr;
+  // ovrfsr_set_focus: `active` once some eye has a focus; then each apply copies its eye's slot block into `focusDev`
+  // ([2][4] words, device) at its head, and the masked kernels read their centre words from there
+  Focus focus;
+  std::atomic<bool> focusActive{false};
+  uint32_t *focusDev = nullptr;
   std::string lastError;
 };
 
@@ -152,6 +173,7 @@ int fail(ovrfsr_ctx *ctx, int status, const char *what, cudaError_t e = cudaSucc
 
 void release_resources(ovrfsr_ctx *c) {
   for (int e = 0; e < 2; ++e) { c->upscaled[e].release(); c->sharpened[e].release(); c->hostStage[e].release(); c->hostLinearIn[e].release(); c->hostLinearOut[e].release(); c->resolved[e].release(); c->expanded[e].release(); }
+  if (c->focusDev) { cudaFree(c->focusDev); c->focusDev = nullptr; }
   if (c->evCreated) {
     for (int i = 0; i < kQueryCount; ++i) { cudaEventDestroy(c->evStart[i]); cudaEventDestroy(c->evEnd[i]); c->evPending[i] = false; }
     c->evCreated = false;
@@ -163,6 +185,46 @@ int select_device(ovrfsr_ctx *c) {
     cudaError_t e = cudaSetDevice(c->cfg.device);
     if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "cudaSetDevice", e);
   }
+  return OVRFSR_OK;
+}
+
+// the slot's words: host::centre_radius with each focused eye's proj_centre pair replaced by its focus (block 1 of a
+// shared texture is never read)
+void write_focus_slot(Focus &f) {
+  if (!f.slot || !f.ready) return;
+  ovrfsr_config cfg = f.cfg;
+  for (int e = 0; e < 2; ++e)
+    if (f.set[e]) { cfg.proj_centre[2 * e] = f.xy[e][0]; cfg.proj_centre[2 * e + 1] = f.xy[e][1]; }
+  for (int b = 0; b < 2; ++b) {
+    alignas(8) uint32_t centre[4], radius[4];
+    host::centre_radius(centre, radius, cfg, b, f.onlyOneEye, f.outW, f.outH);
+    uint64_t pair[2];
+    std::memcpy(pair, centre, sizeof(pair));
+    uint64_t *dst = reinterpret_cast<uint64_t *>(f.slot + 4 * b);
+    __atomic_store_n(&dst[0], pair[0], __ATOMIC_RELAXED);
+    __atomic_store_n(&dst[1], pair[1], __ATOMIC_RELAXED);
+  }
+}
+
+// head of an apply with a focus active: copy this eye's slot block to its device block on `s`, so the kernels of the
+// apply see the focus the slot holds when the copy runs (and a captured graph re-reads the slot on every replay)
+int latch_focus(ovrfsr_ctx *c, int eye, cudaStream_t s, const uint32_t **centreDev) {
+  Focus &f = c->focus;
+  if (!f.slot) {
+    uint32_t *slot = nullptr;
+    cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&slot), 2 * 4 * sizeof(uint32_t), cudaHostAllocPortable);
+    if (e != cudaSuccess) return fail(c, OVRFSR_ERR_NOMEM, "allocating the focus slot", e);
+    std::lock_guard<std::mutex> lock(f.mu);
+    f.slot = slot;
+    write_focus_slot(f);
+  }
+  if (!c->focusDev) {
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&c->focusDev), 2 * 4 * sizeof(uint32_t));
+    if (e != cudaSuccess) { c->focusDev = nullptr; return fail(c, OVRFSR_ERR_NOMEM, "allocating the focus block", e); }
+  }
+  cudaError_t e = cudaMemcpyAsync(c->focusDev + 4 * eye, f.slot + 4 * eye, 4 * sizeof(uint32_t), cudaMemcpyHostToDevice, s);
+  if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "focus copy", e);
+  *centreDev = c->focusDev + 4 * eye;
   return OVRFSR_OK;
 }
 
@@ -214,6 +276,12 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
     }
     c->evCreated = true;
   }
+  { // the focus words for the new config / layout / output size (the focus itself survives resets)
+    std::lock_guard<std::mutex> lock(c->focus.mu);
+    Focus &f = c->focus;
+    f.cfg = c->cfg; f.onlyOneEye = one; f.outW = c->outputWidth; f.outH = c->outputHeight; f.ready = true;
+    write_focus_slot(f);
+  }
   c->initialized = true;
   return OVRFSR_OK;
 }
@@ -241,30 +309,32 @@ int nis_status(cudaError_t e) {
   return (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA;
 }
 
-// fin: the image the apply's last pass writes (EASU's outside-radius groups go there when RCAS follows)
-int run_upscale(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &out, const PassImage &fin, cudaStream_t s) {
+// fin: the image the apply's last pass writes (EASU's outside-radius groups go there when RCAS follows); centreDev: the
+// focus block latched for this apply, or nullptr
+int run_upscale(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &out, const PassImage &fin, cudaStream_t s,
+                const uint32_t *centreDev) {
   const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
   cudaError_t e;
   if (c->cfg.use_nis) {
-    e = launch_nis(false, in, out, c->nisScalerConfig[eye], c->cfg.math_mode, s);
+    e = launch_nis(false, in, out, c->nisScalerConfig[eye], c->cfg.math_mode, s, centreDev);
     return e == cudaSuccess ? OVRFSR_OK : fail(c, nis_status(e), "NIS scaler dispatch", e);
   }
   const PassImage *direct = paired_passes(c) ? &fin : nullptr;
   const float tint = 1.0f - (float)c->sharpenConstants[eye][3] * 0.3f;
-  e = strict ? launch_easu_strict(in, out, c->upscaleConstants[eye], s, direct, tint)
-             : launch_easu_fast(in, out, c->upscaleConstants[eye], s, direct, tint);
+  e = strict ? launch_easu_strict(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev)
+             : launch_easu_fast(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev);
   return e == cudaSuccess ? OVRFSR_OK : fail(c, OVRFSR_ERR_CUDA, "EASU launch", e);
 }
 
-int run_sharpen(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &out, cudaStream_t s) {
+int run_sharpen(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &out, cudaStream_t s, const uint32_t *centreDev) {
   const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
   if (c->cfg.use_nis) {
-    const cudaError_t e = launch_nis(true, in, out, c->nisSharpenConfig[eye], c->cfg.math_mode, s);
+    const cudaError_t e = launch_nis(true, in, out, c->nisSharpenConfig[eye], c->cfg.math_mode, s, centreDev);
     return e == cudaSuccess ? OVRFSR_OK : fail(c, nis_status(e), "NIS sharpen dispatch", e);
   }
   const bool skip = paired_passes(c);
-  cudaError_t e = strict ? launch_rcas_strict(in, out, c->sharpenConstants[eye], s, skip)
-                         : launch_rcas_fast(in, out, c->sharpenConstants[eye], s, skip);
+  cudaError_t e = strict ? launch_rcas_strict(in, out, c->sharpenConstants[eye], s, skip, centreDev)
+                         : launch_rcas_fast(in, out, c->sharpenConstants[eye], s, skip, centreDev);
   return e == cudaSuccess ? OVRFSR_OK : fail(c, OVRFSR_ERR_CUDA, "RCAS launch", e);
 }
 
@@ -291,6 +361,11 @@ int save_capture(ovrfsr_ctx *c, const Image &img, cudaStream_t s) {
 // polling stay in the caller; the F7 capture is served through ovrfsr_request_capture).  dst: the caller's image the
 // last pass writes (ovrfsr_apply_into), else the ctx-owned output.
 int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, const Image *dst, cudaStream_t s) {
+  const uint32_t *centreDev = nullptr;
+  if (c->focusActive.load(std::memory_order_acquire)) {
+    const int rc = latch_focus(c, eye, s, &centreDev);
+    if (rc != OVRFSR_OK) return rc;
+  }
   // GetInputView: array textures keep the right eye in slice 1 (PostProcessor.cpp:254-268)
   const int slice = (src->array_slices > 1 && eye == 1) ? 1 : 0;
   PassImage in = pass_image(*src, slice);
@@ -334,8 +409,8 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
     // two dispatches below
     const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
     const PassImage out2 = pass_image(fin);
-    const cudaError_t e = strict ? launch_fsr_fused_strict(in, out2, c->upscaleConstants[eye], c->sharpenConstants[eye], s)
-                                 : launch_fsr_fused_fast(in, out2, c->upscaleConstants[eye], c->sharpenConstants[eye], s);
+    const cudaError_t e = strict ? launch_fsr_fused_strict(in, out2, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev)
+                                 : launch_fsr_fused_fast(in, out2, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev);
     if (e == cudaSuccess) { fused = true; result = fin; }
     else if (e != cudaErrorInvalidValue && e != cudaErrorInvalidConfiguration) return fail(c, OVRFSR_ERR_CUDA, "fused EASU+RCAS launch", e);
   }
@@ -345,13 +420,13 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
     if (!(last && dst) && !c->upscaled[eye].img.data && !c->upscaled[eye].alloc(c->outputWidth, c->outputHeight, c->outFormat))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
     const Image &up = last && dst ? *dst : c->upscaled[eye].img;
-    int rc = run_upscale(c, eye, in, pass_image(up), pass_image(fin), s);
+    int rc = run_upscale(c, eye, in, pass_image(up), pass_image(fin), s, centreDev);
     if (rc != OVRFSR_OK) return rc;
     in = pass_image(up);
     result = up;
   }
   if (!fused && sharpen_pass(c->cfg)) {
-    int rc = run_sharpen(c, eye, in, pass_image(fin), s);
+    int rc = run_sharpen(c, eye, in, pass_image(fin), s, centreDev);
     if (rc != OVRFSR_OK) return rc;
     result = fin;
   }
@@ -502,6 +577,7 @@ void ovrfsr_destroy(ovrfsr_ctx *ctx) {
     if (ctx->cfg.device >= 0) cudaSetDevice(ctx->cfg.device);
     release_resources(ctx);
   }
+  if (ctx->focus.slot) cudaFreeHost(ctx->focus.slot);
   delete ctx;
 }
 
@@ -528,6 +604,27 @@ int ovrfsr_set_config(ovrfsr_ctx *ctx, const ovrfsr_config *cfg) {
   int rc = ovrfsr_reset(ctx);
   ctx->cfg = *cfg;
   return rc;
+}
+
+int ovrfsr_set_focus(ovrfsr_ctx *ctx, int eye, float x, float y) {
+  if (!ctx || (eye != 0 && eye != 1) || !(x >= 0.f && x <= 1.f) || !(y >= 0.f && y <= 1.f)) return OVRFSR_ERR_INVALID;
+  Focus &f = ctx->focus;
+  std::lock_guard<std::mutex> lock(f.mu);
+  f.set[eye] = true;
+  f.xy[eye][0] = x; f.xy[eye][1] = y;
+  write_focus_slot(f);
+  ctx->focusActive.store(true, std::memory_order_release);
+  return OVRFSR_OK;
+}
+
+int ovrfsr_clear_focus(ovrfsr_ctx *ctx, int eye) {
+  if (!ctx || (eye != 0 && eye != 1)) return OVRFSR_ERR_INVALID;
+  Focus &f = ctx->focus;
+  std::lock_guard<std::mutex> lock(f.mu);
+  f.set[eye] = false;
+  write_focus_slot(f); // graphs captured with a focus fall back to the projection centre
+  ctx->focusActive.store(f.set[0] || f.set[1], std::memory_order_release);
+  return OVRFSR_OK;
 }
 
 int ovrfsr_get_config(const ovrfsr_ctx *ctx, ovrfsr_config *cfg) {

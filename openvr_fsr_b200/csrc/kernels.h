@@ -17,28 +17,37 @@ struct PassImage { void *ptr; uint32_t pitch; int w, h; int format; bool array =
 // apply, EASU writes the outside-radius groups -- which RCAS would only copy (x the debug tint `tintGB`) -- straight
 // to the final image `direct`, and RCAS visits only tiles / groups inside the radius.  Same output bits as two plain
 // dispatches; a stateless dispatch passes nullptr / false.
+// `centreDev` (every masked launcher): nullptr = the imageCentre words of the constant block; else a 16-byte device block
+// the kernels read those four words from when they run (the ctx path with a focus, ovrfsr_set_focus).
 cudaError_t launch_easu_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,
-                             const PassImage *direct = nullptr, float tintGB = 1.0f);
+                             const PassImage *direct = nullptr, float tintGB = 1.0f, const uint32_t *centreDev = nullptr);
 cudaError_t launch_easu_strict(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,
-                               const PassImage *direct = nullptr, float tintGB = 1.0f);
+                               const PassImage *direct = nullptr, float tintGB = 1.0f, const uint32_t *centreDev = nullptr);
 cudaError_t launch_rcas_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[12], cudaStream_t s,
-                             bool skipOutside = false);
+                             bool skipOutside = false, const uint32_t *centreDev = nullptr);
 cudaError_t launch_rcas_strict(const PassImage &src, const PassImage &dst, const uint32_t consts[12], cudaStream_t s,
-                               bool skipOutside = false);
+                               bool skipOutside = false, const uint32_t *centreDev = nullptr);
 
 // EASU -> RCAS in one kernel (fsr_fused.cuh): ku = UpscaleConstants, ks = SharpenConstants; dst.format (RGBA8, or RGB10A2
 // for an RGB10A2 source) is also the format the intermediate is quantised to.  cudaErrorInvalidValue /
 // cudaErrorInvalidConfiguration = this pair of passes cannot be fused (the caller runs the two dispatches instead).
-cudaError_t launch_fsr_fused_fast(const PassImage &src, const PassImage &dst, const uint32_t ku[24], const uint32_t ks[12], cudaStream_t s);
-cudaError_t launch_fsr_fused_strict(const PassImage &src, const PassImage &dst, const uint32_t ku[24], const uint32_t ks[12], cudaStream_t s);
+cudaError_t launch_fsr_fused_fast(const PassImage &src, const PassImage &dst, const uint32_t ku[24], const uint32_t ks[12], cudaStream_t s,
+                                  const uint32_t *centreDev = nullptr);
+cudaError_t launch_fsr_fused_strict(const PassImage &src, const PassImage &dst, const uint32_t ku[24], const uint32_t ks[12], cudaStream_t s,
+                                    const uint32_t *centreDev = nullptr);
 
 // NIS (nis_kernels.cuh).  cfg = the 256-byte NISConfig block; coef = [2][64][8] floats (scale, usm) on the host.
-cudaError_t launch_nis_scaler_fast(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s);
-cudaError_t launch_nis_scaler_strict(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s);
-cudaError_t launch_nis_sharpen_fast(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s);
-cudaError_t launch_nis_sharpen_strict(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s);
+cudaError_t launch_nis_scaler_fast(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
+                                   const uint32_t *centreDev = nullptr);
+cudaError_t launch_nis_scaler_strict(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
+                                     const uint32_t *centreDev = nullptr);
+cudaError_t launch_nis_sharpen_fast(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
+                                    const uint32_t *centreDev = nullptr);
+cudaError_t launch_nis_sharpen_strict(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
+                                      const uint32_t *centreDev = nullptr);
 // NVScaler (sharpenOnly false) or NVSharpen with this library's filter banks, on images already validated (nis_capi.cu)
-cudaError_t launch_nis(bool sharpenOnly, const PassImage &src, const PassImage &dst, const void *cfg256, int mathMode, cudaStream_t s);
+cudaError_t launch_nis(bool sharpenOnly, const PassImage &src, const PassImage &dst, const void *cfg256, int mathMode, cudaStream_t s,
+                       const uint32_t *centreDev = nullptr);
 
 // legacy CAS (cas_kernels.cuh).  consts = const0, const1 of src/cas/cas.compute.h:1-4 as CasSetup fills them.
 cudaError_t launch_cas_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[8], int sharpenOnly, cudaStream_t s);

@@ -56,14 +56,16 @@ int status_of(cudaError_t e) {
 } // namespace
 
 cudaError_t ovrfsr::launch_nis(bool sharpenOnly, const PassImage &src, const PassImage &dst, const void *cfg256, int mathMode,
-                               cudaStream_t s) {
+                               cudaStream_t s, const uint32_t *centreDev) {
   const bool strict = mathMode == OVRFSR_MATH_STRICT;
-  if (sharpenOnly) return strict ? launch_nis_sharpen_strict(src, dst, cfg256, nullptr, s) : launch_nis_sharpen_fast(src, dst, cfg256, nullptr, s);
+  if (sharpenOnly)
+    return strict ? launch_nis_sharpen_strict(src, dst, cfg256, nullptr, s, centreDev) : launch_nis_sharpen_fast(src, dst, cfg256, nullptr, s, centreDev);
   const float *coef = ovrfsr_nis_coef_scale(); // g_coefScale and g_coefUsm are contiguous? no: upload buffer below
   static float both[2][64 * 8];
   static std::once_flag once;
   std::call_once(once, [&] { std::memcpy(both[0], coef, sizeof(both[0])); std::memcpy(both[1], ovrfsr_nis_coef_usm(), sizeof(both[1])); });
-  return strict ? launch_nis_scaler_strict(src, dst, cfg256, &both[0][0], s) : launch_nis_scaler_fast(src, dst, cfg256, &both[0][0], s);
+  return strict ? launch_nis_scaler_strict(src, dst, cfg256, &both[0][0], s, centreDev)
+                : launch_nis_scaler_fast(src, dst, cfg256, &both[0][0], s, centreDev);
 }
 
 extern "C" {

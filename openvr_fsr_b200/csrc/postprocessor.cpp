@@ -56,7 +56,11 @@ void PostProcessor::Apply(EVREye eEye, const Texture_t *pTexture, const VRTextur
   if (!initialized) {
     // the reference re-reads the Config singleton whenever it (re)creates resources
     const ovrfsr_config k = config_from_singleton();
-    int rc = ctx ? ovrfsr_set_config(ctx, &k) : ovrfsr_create(&ctx, &k);
+    int rc;
+    {
+      std::lock_guard<std::mutex> lock(ctxMutex); // SetFocus may create the ctx from another thread
+      rc = ctx ? ovrfsr_set_config(ctx, &k) : ovrfsr_create(&ctx, &k);
+    }
     if (rc != OVRFSR_OK) {
       Log() << "Resource creation failed, disabling (" << ovrfsr_status_string(rc) << ")\n";
       enabled = false;
@@ -120,5 +124,25 @@ void PostProcessor::TakeCapture(const char *directory) {
 }
 
 bool PostProcessor::GetAverageGpuTimeMs(float *ms) { return ctx && ovrfsr_get_gpu_time_ms(ctx, ms) > 0; }
+
+ovrfsr_ctx *PostProcessor::Context() {
+  std::lock_guard<std::mutex> lock(ctxMutex);
+  if (!ctx) {
+    const ovrfsr_config k = config_from_singleton();
+    if (ovrfsr_create(&ctx, &k) != OVRFSR_OK) ctx = nullptr;
+  }
+  return ctx;
+}
+
+// the focus lives in the ctx and survives the set_config of the first Apply and every Reset
+bool PostProcessor::SetFocus(EVREye eEye, float x, float y) {
+  ovrfsr_ctx *c = Context();
+  return c && ovrfsr_set_focus(c, eEye == Eye_Right ? 1 : 0, x, y) == OVRFSR_OK;
+}
+
+bool PostProcessor::ClearFocus(EVREye eEye) {
+  ovrfsr_ctx *c = Context();
+  return c && ovrfsr_clear_focus(c, eEye == Eye_Right ? 1 : 0) == OVRFSR_OK;
+}
 
 } // namespace vr

@@ -8,6 +8,7 @@
 #pragma once
 
 #include <iosfwd>
+#include <mutex>
 
 #include "../../include/ovrfsr.h"
 #include "config.h"
@@ -42,8 +43,16 @@ public:
     outputTargets[0] = left;
     outputTargets[1] = right;
   }
+  // Foveation (ovrfsr_set_focus / ovrfsr_clear_focus): the radius mask of `eEye` centres on (x, y) in that eye's
+  // normalised texture coordinates instead of its projection centre, from the next frame whose GPU work starts after
+  // the call.  Callable from any thread (e.g. the eye tracker's), before the first Apply too.  false: rejected
+  // (x / y not finite or outside [0, 1]).
+  bool SetFocus(EVREye eEye, float x, float y);
+  bool ClearFocus(EVREye eEye);
 
 private:
+  ovrfsr_ctx *Context(); // creates the ctx on first use (no GPU work); guarded by ctxMutex
+  std::mutex ctxMutex;
   bool enabled = true;
   bool initialized = false;
   bool inputIsSrgb = false;
