@@ -138,6 +138,23 @@ typedef struct ovrfsr_config {
  * recomputed ring and lower occupancy make it slower than the two dispatches (DESIGN.md section 5).  Default (bit clear): the reference's two dispatches (PostProcessor.cpp:586-594),
  * with the outside-radius pixels written straight to the final image by the first one. */
 #define OVRFSR_FLAG_FUSED_FSR 1
+/* HDR float eye textures through AMD's simple reversible tone mapper (ffx_fsr1.h: FsrSrtmF / FsrSrtmInvF), an extension
+ * the reference never enables.  EASU's luma analysis and RCAS's limiter assume display-referred values in [0, 1]; with
+ * linear HDR input (scRGB, highlights above 1) the limiter's bound hitMax = (1 - mx) / (4 mn - 4) no longer prevents
+ * overshoot.  With this bit the FSR passes run on
+ *   F(c) = c / (max3(c.rgb) + 1)                      [0, 65504] -> [0, 0.9999848]
+ * and the last one maps its result back with
+ *   G(c) = c / max(1/32768, 1 - max3(c.rgb))          so G(c) <= 32768 x max3(c.rgb): the peak is 32768
+ * (alpha untouched, IEEE reciprocal in both math modes).  It takes effect on the FSR path with a float source (RGBA16F,
+ * RGBA32F, RGB32F after its expansion, a multisampled one after its resolve) and is ignored -- same output bits as with
+ * the bit clear -- for UNORM sources and for use_nis.  With both passes the intermediate is RGBA32F for a float output
+ * and RGBA16F for a UNORM output (an FP16 tone-mapped value near 1 is too coarse for HDR output once G amplifies it,
+ * irrelevant where the output clips at 1; DESIGN.md section 4); the pairing and OVRFSR_FLAG_FUSED_FSR do not apply.  With
+ * RCAS alone the outside-radius copy also runs in tone-mapped space (G(tint x F(c))): close to a copy, not bit-exact.
+ * Negative, NaN and infinite channels are outside the tone map's domain: they go through the same formula and get
+ * whatever IEEE arithmetic gives (e.g. max3 = -1 divides by zero).  Changing the bit through ovrfsr_set_config resets
+ * the ctx like any config change. */
+#define OVRFSR_FLAG_SRTM 2
 
 typedef struct ovrfsr_ctx ovrfsr_ctx;
 
@@ -223,6 +240,17 @@ OVRFSR_API int ovrfsr_dispatch_fsr_easu(const ovrfsr_image *src, const ovrfsr_im
 /* g_FSRSharpenShader: consts = SharpenConstants, 12 x u32 (PostProcessor.cpp:403-407) */
 OVRFSR_API int ovrfsr_dispatch_fsr_rcas(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[12],
                                         int math_mode, void *stream);
+/* The two dispatches above with the tone map of OVRFSR_FLAG_SRTM per pass (pass_flags, OR of the bits below), for hosts
+ * that chain the passes themselves: F after the decode of every texel the pass reads, G before the encode of every pixel
+ * it stores.  The ctx's chain is EASU with SRTM_IN into an RGBA16F / RGBA32F image, then RCAS with SRTM_OUT (RCAS alone:
+ * both).  pass_flags == 0 launches exactly what ovrfsr_dispatch_fsr_easu / _rcas launch.  OVRFSR_ERR_UNSUPPORTED for
+ * either bit with a UNORM source, OVRFSR_ERR_INVALID for unknown bits. */
+#define OVRFSR_PASS_SRTM_IN 1
+#define OVRFSR_PASS_SRTM_OUT 2
+OVRFSR_API int ovrfsr_dispatch_fsr_easu_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[24],
+                                           int math_mode, int pass_flags, void *stream);
+OVRFSR_API int ovrfsr_dispatch_fsr_rcas_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[12],
+                                           int math_mode, int pass_flags, void *stream);
 /* g_FSRUpscaleShader followed by g_FSRSharpenShader (ApplyPostProcess, PostProcessor.cpp:586-594) as ONE kernel: the
  * upscaled image is quantised to dst->format (RGBA8, or RGB10A2 for an RGB10A2 source) exactly as the first dispatch
  * stores it, but never leaves shared memory.  Bit-identical to the two dispatches above run back to back.  The two

@@ -18,6 +18,8 @@ FORMAT_SRGB_BIT, FORMAT_TYPELESS_BIT, FORMAT_LAYOUT_MASK = 0x100, 0x200, 0xff
 FORMAT_ARRAY_BIT = 0x400  # data is a cudaArray_t
 MATH_FAST, MATH_STRICT = 0, 1
 FLAG_FUSED_FSR = 1
+FLAG_SRTM = 2  # AMD's reversible tone map around the FSR passes of a float source
+PASS_SRTM_IN, PASS_SRTM_OUT = 1, 2  # pass_flags of ovrfsr_dispatch_fsr_easu_ex / _rcas_ex
 
 
 class Image(C.Structure):
@@ -51,6 +53,8 @@ SYMBOLS = {
     "ovrfsr_clear_focus": (C.c_int, [_vp, C.c_int]),
     "ovrfsr_dispatch_fsr_easu": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, _vp]),
     "ovrfsr_dispatch_fsr_rcas": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, _vp]),
+    "ovrfsr_dispatch_fsr_easu_ex": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, C.c_int, _vp]),
+    "ovrfsr_dispatch_fsr_rcas_ex": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, C.c_int, _vp]),
     "ovrfsr_dispatch_fsr_fused": (C.c_int, [_imgp, _imgp, _u32p, _u32p, C.c_int, _vp]),
     "ovrfsr_dispatch_nis_scaler": (C.c_int, [_imgp, _imgp, _vp, C.c_int, _vp]),
     "ovrfsr_dispatch_nis_sharpen": (C.c_int, [_imgp, _imgp, _vp, C.c_int, _vp]),

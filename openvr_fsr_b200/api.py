@@ -29,6 +29,7 @@ class Config:
     outputFormat: int = L.FORMAT_AUTO
     mathMode: int = L.MATH_STRICT
     fusedFsr: bool = False  # OVRFSR_FLAG_FUSED_FSR: one fused EASU->RCAS kernel instead of the two dispatches
+    srtm: bool = False      # OVRFSR_FLAG_SRTM: FSR on a float (HDR) source runs between AMD's reversible tone map and its inverse
 
     def to_c(self) -> L.Config:
         c = L.Config()
@@ -38,7 +39,7 @@ class Config:
         c.debug_mode = int(self.debugMode)
         c.proj_centre = (C.c_float * 4)(*self.projCentre)
         c.device, c.output_format, c.math_mode = self.device, self.outputFormat, self.mathMode
-        c.flags = L.FLAG_FUSED_FSR if self.fusedFsr else 0
+        c.flags = (L.FLAG_FUSED_FSR if self.fusedFsr else 0) | (L.FLAG_SRTM if self.srtm else 0)
         return c
 
 
@@ -331,13 +332,32 @@ def _dispatch(fn, src, dst, consts, math_mode, stream, src_fmt=None, dst_fmt=Non
     return dst
 
 
-def fsr_easu(src, dst, consts24, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None):
+def _pass_flags(srtm_in, srtm_out):
+    return (L.PASS_SRTM_IN if srtm_in else 0) | (L.PASS_SRTM_OUT if srtm_out else 0)
+
+
+def _dispatch_ex(fn, src, dst, consts, math_mode, flags, stream, src_fmt=None, dst_fmt=None):
+    s, d = image_of(src, src_fmt), image_of(dst, dst_fmt)
+    L.check(fn(C.byref(s), C.byref(d), consts, math_mode, flags, _stream_ptr(stream)), fn.__name__)
+    return dst
+
+
+def fsr_easu(src, dst, consts24, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False):
+    """g_FSRUpscaleShader.  srtm_in / srtm_out (float sources only): AMD's reversible tone map on every texel read / its
+    inverse on every pixel stored (ovrfsr_dispatch_fsr_easu_ex)"""
     c = (C.c_uint32 * 24)(*[int(x) for x in consts24])
+    if srtm_in or srtm_out:
+        return _dispatch_ex(L.lib().ovrfsr_dispatch_fsr_easu_ex, src, dst, c, math_mode, _pass_flags(srtm_in, srtm_out), stream,
+                            src_fmt, dst_fmt)
     return _dispatch(L.lib().ovrfsr_dispatch_fsr_easu, src, dst, c, math_mode, stream, src_fmt, dst_fmt)
 
 
-def fsr_rcas(src, dst, consts12, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None):
+def fsr_rcas(src, dst, consts12, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False):
+    """g_FSRSharpenShader.  srtm_in / srtm_out as for fsr_easu (ovrfsr_dispatch_fsr_rcas_ex)"""
     c = (C.c_uint32 * 12)(*[int(x) for x in consts12])
+    if srtm_in or srtm_out:
+        return _dispatch_ex(L.lib().ovrfsr_dispatch_fsr_rcas_ex, src, dst, c, math_mode, _pass_flags(srtm_in, srtm_out), stream,
+                            src_fmt, dst_fmt)
     return _dispatch(L.lib().ovrfsr_dispatch_fsr_rcas, src, dst, c, math_mode, stream, src_fmt, dst_fmt)
 
 

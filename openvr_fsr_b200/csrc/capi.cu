@@ -231,9 +231,17 @@ int latch_focus(ovrfsr_ctx *c, int eye, cudaStream_t s, const uint32_t **centreD
 bool upscale_pass(const ovrfsr_config &cfg) { return cfg.render_scale != 1.f; }                    // PostProcessor.cpp:586
 bool sharpen_pass(const ovrfsr_config &cfg) { return !cfg.use_nis || cfg.render_scale == 1.f; }    // PostProcessor.cpp:591
 // both FSR passes run and the caller opted into the fused kernel (the intermediate is then never materialised)
-bool fused_pass(const ovrfsr_config &cfg) {
-  return !cfg.use_nis && upscale_pass(cfg) && sharpen_pass(cfg) && (cfg.flags & OVRFSR_FLAG_FUSED_FSR);
+// OVRFSR_FLAG_SRTM takes effect on the FSR path with a float source (an RGB32F one is read through its RGBA32F copy, a
+// multisampled one after its resolve); UNORM sources are display-referred already and NIS has HDR modes of its own
+bool srtm_source(int fmt) { return fmt == OVRFSR_FORMAT_RGBA16F || fmt == OVRFSR_FORMAT_RGBA32F || fmt == OVRFSR_FORMAT_RGB32F; }
+bool srtm_pass(const ovrfsr_config &cfg, int inFormat) { return (cfg.flags & OVRFSR_FLAG_SRTM) && !cfg.use_nis && srtm_source(inFormat); }
+bool fused_pass(const ovrfsr_config &cfg, int inFormat) {
+  return !cfg.use_nis && upscale_pass(cfg) && sharpen_pass(cfg) && (cfg.flags & OVRFSR_FLAG_FUSED_FSR) && !srtm_pass(cfg, inFormat);
 }
+// Format of the upscaled image.  The reference's rule is the output format; with SRTM, EASU stores tone-mapped values
+// that RCAS's G amplifies by up to 32768 near 1, so the intermediate keeps them as RGBA32F for a float output, and as
+// RGBA16F for a UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).
+int mid_format(const ovrfsr_ctx *c);
 
 // PostProcessor::PrepareResources, PostProcessor.cpp:498-561
 int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
@@ -262,8 +270,8 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
                            c->outputHeight);
     // the upscaled image only exists when the two dispatches run (the fused kernel keeps it in shared memory; if a
     // shape turns out not to be fusable it is allocated on first use)
-    const bool wantMid = upscale_pass(c->cfg) && !(fused_pass(c->cfg) && (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2));
-    if (wantMid && !c->upscaled[e].alloc(c->outputWidth, c->outputHeight, c->outFormat))
+    const bool wantMid = upscale_pass(c->cfg) && !(fused_pass(c->cfg, c->inFormat) && (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2));
+    if (wantMid && !c->upscaled[e].alloc(c->outputWidth, c->outputHeight, mid_format(c)))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
     if (sharpen_pass(c->cfg) && !c->sharpened[e].alloc(c->outputWidth, c->outputHeight, c->outFormat))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating sharpened texture", cudaGetLastError());
@@ -302,7 +310,12 @@ void harvest_queries(ovrfsr_ctx *c) {
 bool paired_passes(const ovrfsr_ctx *c) {
   static const bool off = getenv("OVRFSR_NO_PAIR") != nullptr; // dev A/B switch
   return !off && !c->cfg.use_nis && upscale_pass(c->cfg) && sharpen_pass(c->cfg) &&
-         (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2);
+         (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2) && !srtm_pass(c->cfg, c->inFormat);
+}
+
+int mid_format(const ovrfsr_ctx *c) {
+  if (!srtm_pass(c->cfg, c->inFormat) || !sharpen_pass(c->cfg)) return c->outFormat;
+  return (c->outFormat == OVRFSR_FORMAT_RGBA16F || c->outFormat == OVRFSR_FORMAT_RGBA32F) ? OVRFSR_FORMAT_RGBA32F : OVRFSR_FORMAT_RGBA16F;
 }
 
 int nis_status(cudaError_t e) {
@@ -321,8 +334,11 @@ int run_upscale(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &ou
   }
   const PassImage *direct = paired_passes(c) ? &fin : nullptr;
   const float tint = 1.0f - (float)c->sharpenConstants[eye][3] * 0.3f;
-  e = strict ? launch_easu_strict(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev)
-             : launch_easu_fast(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev);
+  // SRTM: F on read; the tone-mapped result goes to the intermediate and RCAS maps it back (RCAS always follows EASU
+  // on the FSR path)
+  const int srtm = srtm_pass(c->cfg, c->inFormat) ? OVRFSR_PASS_SRTM_IN : 0;
+  e = strict ? launch_easu_strict(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev, srtm)
+             : launch_easu_fast(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev, srtm);
   return e == cudaSuccess ? OVRFSR_OK : fail(c, OVRFSR_ERR_CUDA, "EASU launch", e);
 }
 
@@ -333,8 +349,11 @@ int run_sharpen(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &ou
     return e == cudaSuccess ? OVRFSR_OK : fail(c, nis_status(e), "NIS sharpen dispatch", e);
   }
   const bool skip = paired_passes(c);
-  cudaError_t e = strict ? launch_rcas_strict(in, out, c->sharpenConstants[eye], s, skip, centreDev)
-                         : launch_rcas_fast(in, out, c->sharpenConstants[eye], s, skip, centreDev);
+  // SRTM: G on store; F on read too when RCAS is the only pass (after EASU its source is tone-mapped already)
+  const int srtm = !srtm_pass(c->cfg, c->inFormat) ? 0
+                   : OVRFSR_PASS_SRTM_OUT | (upscale_pass(c->cfg) ? 0 : OVRFSR_PASS_SRTM_IN);
+  cudaError_t e = strict ? launch_rcas_strict(in, out, c->sharpenConstants[eye], s, skip, centreDev, srtm)
+                         : launch_rcas_fast(in, out, c->sharpenConstants[eye], s, skip, centreDev, srtm);
   return e == cudaSuccess ? OVRFSR_OK : fail(c, OVRFSR_ERR_CUDA, "RCAS launch", e);
 }
 
@@ -404,7 +423,7 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
   const Image &fin = dst ? *dst : c->sharpened[eye].img;
   bool fused = false;
   // the fused kernel has no array I/O: with an array source or destination the two dispatches run
-  if (fused_pass(c->cfg) && (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2) && !src->array && !fin.array) {
+  if (fused_pass(c->cfg, c->inFormat) && (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2) && !src->array && !fin.array) {
     // ApplyUpscaling + ApplySharpening (PostProcessor.cpp:586-594) as one kernel; shapes it does not cover take the
     // two dispatches below
     const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
@@ -417,7 +436,7 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
   if (!fused && upscale_pass(c->cfg)) {
     // without a sharpening pass the upscaled image is the output
     const bool last = !sharpen_pass(c->cfg);
-    if (!(last && dst) && !c->upscaled[eye].img.data && !c->upscaled[eye].alloc(c->outputWidth, c->outputHeight, c->outFormat))
+    if (!(last && dst) && !c->upscaled[eye].img.data && !c->upscaled[eye].alloc(c->outputWidth, c->outputHeight, mid_format(c)))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
     const Image &up = last && dst ? *dst : c->upscaled[eye].img;
     int rc = run_upscale(c, eye, in, pass_image(up), pass_image(fin), s, centreDev);
@@ -777,14 +796,26 @@ struct DispatchPair {
 
 int ovrfsr_dispatch_fsr_easu(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t consts[24], int math_mode,
                              void *stream) {
+  return ovrfsr_dispatch_fsr_easu_ex(src_tagged, dst_tagged, consts, math_mode, 0, stream);
+}
+
+// the pass flags of a stateless FSR dispatch: OVRFSR_OK, or the status to return (checked after the image pair)
+static int check_pass_flags(const Image *src, int pass_flags) {
+  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT)) return OVRFSR_ERR_INVALID;
+  if (pass_flags && src->format != OVRFSR_FORMAT_RGBA16F && src->format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
+  return OVRFSR_OK;
+}
+
+int ovrfsr_dispatch_fsr_easu_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t consts[24], int math_mode,
+                                int pass_flags, void *stream) {
   const DispatchPair io(src_tagged, dst_tagged);
   const Image *src = io.src, *dst = io.dst;
   if (!consts) return OVRFSR_ERR_INVALID;
   int rc = check_pair(src, dst);
-  if (rc != OVRFSR_OK) return rc;
+  if (rc != OVRFSR_OK || (rc = check_pass_flags(src, pass_flags)) != OVRFSR_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_easu_strict(pass_image(*src), pass_image(*dst), consts, s)
-                                                  : launch_easu_fast(pass_image(*src), pass_image(*dst), consts, s);
+  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_easu_strict(pass_image(*src), pass_image(*dst), consts, s, nullptr, 1.0f, nullptr, pass_flags)
+                                                  : launch_easu_fast(pass_image(*src), pass_image(*dst), consts, s, nullptr, 1.0f, nullptr, pass_flags);
   if (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) return OVRFSR_ERR_UNSUPPORTED;
   return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
 }
@@ -807,15 +838,20 @@ int ovrfsr_dispatch_fsr_fused(const ovrfsr_image *src_tagged, const ovrfsr_image
 
 int ovrfsr_dispatch_fsr_rcas(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t consts[12], int math_mode,
                              void *stream) {
+  return ovrfsr_dispatch_fsr_rcas_ex(src_tagged, dst_tagged, consts, math_mode, 0, stream);
+}
+
+int ovrfsr_dispatch_fsr_rcas_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t consts[12], int math_mode,
+                                int pass_flags, void *stream) {
   const DispatchPair io(src_tagged, dst_tagged);
   const Image *src = io.src, *dst = io.dst;
   if (!consts) return OVRFSR_ERR_INVALID;
   int rc = check_pair(src, dst);
-  if (rc != OVRFSR_OK) return rc;
+  if (rc != OVRFSR_OK || (rc = check_pass_flags(src, pass_flags)) != OVRFSR_OK) return rc;
   if (src->width != dst->width || src->height != dst->height) return OVRFSR_ERR_INVALID;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_rcas_strict(pass_image(*src), pass_image(*dst), consts, s)
-                                                  : launch_rcas_fast(pass_image(*src), pass_image(*dst), consts, s);
+  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_rcas_strict(pass_image(*src), pass_image(*dst), consts, s, false, nullptr, pass_flags)
+                                                  : launch_rcas_fast(pass_image(*src), pass_image(*dst), consts, s, false, nullptr, pass_flags);
   if (e == cudaErrorInvalidValue) return OVRFSR_ERR_UNSUPPORTED;
   return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
 }

@@ -41,6 +41,7 @@ struct EasuArgs {
   // intermediate `dst` only where an edge-adjacent group is inside the radius (RCAS reads one pixel across the edge).
   ImageRW direct;           // ptr == nullptr: plain dispatch
   float tintGB;             // 1 - debug*0.3 of the following RCAS pass
+  int srtmIn, srtmOut;      // float sources only: srtm_fwd on every texel read / srtm_inv on every pixel stored
 };
 
 struct RcasArgs {
@@ -53,7 +54,23 @@ struct RcasArgs {
   uint32_t radiusSq;
   int skipOutside;          // the preceding EASU launch already wrote the outside-radius groups to dst (EasuArgs::direct)
   int opaqueSrc;            // B8G8R8X8 source: the X byte reads as alpha 1 (only the outside-radius copy looks at alpha)
+  int srtmIn, srtmOut;      // float sources only: srtm_fwd on every texel read / srtm_inv on every pixel stored
 };
+
+// AMD's simple reversible tone mapper (ffx_fsr1.h, FsrSrtmF / FsrSrtmInvF), the opt-in HDR extension of both passes:
+// F(c) = c / (max3(c.rgb) + 1) maps linear [0, FP16_MAX] into [0, 1), where EASU's luma analysis and RCAS's limiter
+// are valid; G(c) = c / max(1/32768, 1 - max3(c.rgb)) maps back (peak 32768).  Alpha is untouched.  IEEE reciprocal in
+// both math modes: G amplifies any error near 1.  Texels outside F's domain (negative, NaN, +-inf, max3 <= -1) go
+// through the same formula; what IEEE arithmetic gives is the result.  max3 uses fmaxf, the pinned min / max rule, so
+// the operand order does not matter.  Only float-source instantiations ever contain these (if constexpr on FIN).
+__device__ __forceinline__ void srtm_fwd(float &r, float &g, float &b) {
+  const float k = __frcp_rn(__fadd_rn(fmaxf(fmaxf(r, g), b), 1.0f));
+  r = __fmul_rn(r, k); g = __fmul_rn(g, k); b = __fmul_rn(b, k);
+}
+__device__ __forceinline__ void srtm_inv(float &r, float &g, float &b) {
+  const float k = __frcp_rn(fmaxf((float)(1.0 / 32768.0), __fsub_rn(1.0f, fmaxf(fmaxf(r, g), b))));
+  r = __fmul_rn(r, k); g = __fmul_rn(g, k); b = __fmul_rn(b, k);
+}
 
 // out pixel -> source position; the same instruction sequence is used for the tile origin and
 // for every pixel so that both agree to the bit.
@@ -474,6 +491,9 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
       const int ty = (int)__umulhi((uint32_t)q, colsRcp), tx = q - ty * cols;
       const int gy = clampi(sy0 + ty, 0, a.src.h - 1), gx = clampi(tx0 + tx, 0, a.src.w - 1);
       float4 c = get_texel<FIN, ANYIO>(a.src, io.src, gx, gy);
+      if constexpr (!packed32(FIN)) {
+        if (a.srtmIn) srtm_fwd(c.x, c.y, c.z); // the tile, the features and the bilinear fallback all see F(texel)
+      }
       sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y);
       c.w = 1.0f; // EASU ignores source alpha; the fast path accumulates the tap weight through this lane
       sC[ty * TW + tx] = c;
@@ -550,6 +570,9 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
         float3 c;
         if constexpr (kStrict) c = easu_filter<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
         else c = easu_filter_fast<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
+        if constexpr (!packed32(FIN)) {
+          if (a.srtmOut) srtm_inv(c.x, c.y, c.z);
+        }
         if constexpr (ANYIO) {
           put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
         } else {
@@ -563,7 +586,10 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
       for (int k = 0; k < 8; ++k) {
         const int y = yFirst + 2 * k;
         if (y >= a.dst.h) break;
-        const float3 c = easu_bilinear(sC, TW, ax, sRowAxis[y - oy0]);
+        float3 c = easu_bilinear(sC, TW, ax, sRowAxis[y - oy0]);
+        if constexpr (!packed32(FIN)) {
+          if (a.srtmOut) srtm_inv(c.x, c.y, c.z); // never with `direct`: the launcher rejects SRTM on a paired launch
+        }
         if (mid) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
         if constexpr (direct) {
           if (a.tintGB == 1.0f) {
@@ -778,6 +804,10 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
           c = get_texel<FIN, ANYIO>(a.src, io.src, gx, gy);
         }
         if constexpr (OPQ) c.w = 1.0f;
+        // FsrRcasInputF, the hook the reference leaves empty.  The zeros outside the image need no map: F(+0) = +0.
+        if constexpr (!packed32(FIN)) {
+          if (a.srtmIn) srtm_fwd(c.x, c.y, c.z);
+        }
       }
       sC[ty * kRcasTW + tx] = c;
     }
@@ -803,7 +833,10 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       const int y = y0 + k;
       if (y >= a.dst.h) break;
       const float4 h = p[kRcasTW], d = p[-1], f = p[1];
-      const float3 c = rcas_filter_mode<FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_BGRA8>(b, d, e, f, h, a.sharp);
+      float3 c = rcas_filter_mode<FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_BGRA8>(b, d, e, f, h, a.sharp);
+      if constexpr (!packed32(FIN)) {
+        if (a.srtmOut) srtm_inv(c.x, c.y, c.z); // also the value a one-colour group's other rows take
+      }
       if constexpr (ANYIO) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
       else *reinterpret_cast<texel_t<FOUT> *>(out) = encode_opaque<FOUT>(c.x, c.y, c.z);
       if (k == 0 && flat) {
@@ -843,7 +876,11 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       const int y = y0 + k;
       if (y >= a.dst.h) break;
       const float4 e = p[k * kRcasTW];
-      put_texel<FOUT, ANYIO>(a.dst, io.dst, x, y, 1.0f * e.x, a.tintGB * e.y, a.tintGB * e.z, 1.0f * e.w);
+      float r = 1.0f * e.x, g = a.tintGB * e.y, bl = a.tintGB * e.z;
+      if constexpr (!packed32(FIN)) {
+        if (a.srtmOut) srtm_inv(r, g, bl); // the copy runs in tone-mapped space: G(tint x F(texel)), alpha as is
+      }
+      put_texel<FOUT, ANYIO>(a.dst, io.dst, x, y, r, g, bl, 1.0f * e.w);
     }
   }
 }

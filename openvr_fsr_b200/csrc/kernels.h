@@ -19,14 +19,18 @@ struct PassImage { void *ptr; uint32_t pitch; int w, h; int format; bool array =
 // dispatches; a stateless dispatch passes nullptr / false.
 // `centreDev` (every masked launcher): nullptr = the imageCentre words of the constant block; else a 16-byte device block
 // the kernels read those four words from when they run (the ctx path with a focus, ovrfsr_set_focus).
+// `srtm` (EASU and RCAS): OVRFSR_PASS_SRTM_* bits, AMD's reversible tone map on the texels read / the pixels stored.
+// Float sources only, and never together with the pairing: cudaErrorInvalidValue otherwise.
 cudaError_t launch_easu_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,
-                             const PassImage *direct = nullptr, float tintGB = 1.0f, const uint32_t *centreDev = nullptr);
+                             const PassImage *direct = nullptr, float tintGB = 1.0f, const uint32_t *centreDev = nullptr,
+                             int srtm = 0);
 cudaError_t launch_easu_strict(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,
-                               const PassImage *direct = nullptr, float tintGB = 1.0f, const uint32_t *centreDev = nullptr);
+                               const PassImage *direct = nullptr, float tintGB = 1.0f, const uint32_t *centreDev = nullptr,
+                               int srtm = 0);
 cudaError_t launch_rcas_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[12], cudaStream_t s,
-                             bool skipOutside = false, const uint32_t *centreDev = nullptr);
+                             bool skipOutside = false, const uint32_t *centreDev = nullptr, int srtm = 0);
 cudaError_t launch_rcas_strict(const PassImage &src, const PassImage &dst, const uint32_t consts[12], cudaStream_t s,
-                               bool skipOutside = false, const uint32_t *centreDev = nullptr);
+                               bool skipOutside = false, const uint32_t *centreDev = nullptr, int srtm = 0);
 
 // EASU -> RCAS in one kernel (fsr_fused.cuh): ku = UpscaleConstants, ks = SharpenConstants; dst.format (RGBA8, or RGB10A2
 // for an RGB10A2 source) is also the format the intermediate is quantised to.  cudaErrorInvalidValue /
