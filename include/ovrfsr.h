@@ -221,16 +221,31 @@ OVRFSR_API int ovrfsr_apply_pair_into(ovrfsr_ctx *ctx, const ovrfsr_image *src_l
  * eye's projection centre in the imageCentre words; the radius is unchanged.  No reset, no reallocation.
  * May be called from any thread, concurrently with the ctx's apply calls.  OVRFSR_ERR_INVALID for
  * eye not in {0,1} or x/y not finite or outside [0,1].
- * Late-latched: while some eye has a focus, each apply (every ovrfsr_apply* entry) starts with a 16-byte
- * host->device copy of its eye's centre words on its stream, and the masked kernels read them from device
- * memory, so a frame uses the focus set before that copy RUNS; a captured CUDA graph follows later calls on
- * every replay.  Each (x, y) pair is published with one 64-bit store: a copy that overlaps an update may mix
- * the two centre pairs of a block, never the x of one update with the y of another.  The focus survives
- * ovrfsr_reset, ovrfsr_set_config and source-size changes.  Host memory only: no CUDA call, no device needed. */
+ * Late-latched: while some eye has a focus or a focus radius (below), each apply (every ovrfsr_apply* entry)
+ * starts with a 32-byte host->device copy of its eye's mask words (imageCentre[4], the squared radius of each
+ * centre pair, two words of padding) on its stream, and the masked kernels read them from device memory, so a
+ * frame uses the focus set before that copy RUNS; a captured CUDA graph follows later calls on every replay.
+ * Each (x, y) pair, and the pair of radius words, is published with one 64-bit store: a copy that overlaps an
+ * update may combine the centre pairs of one update with the radius words of another, each of them whole --
+ * never the x of one update with the y of another -- and every such combination is a valid set of mask words.
+ * The focus survives ovrfsr_reset, ovrfsr_set_config and source-size changes.  Host memory only: no CUDA
+ * call, no device needed. */
 OVRFSR_API int ovrfsr_set_focus(ovrfsr_ctx *ctx, int eye, float x, float y);
-/* Back to the projection centre for `eye` (the reference's behaviour).  Graphs captured with a focus read the
- * projection centre from then on; once no eye has a focus, applies stop issuing the copy. */
+/* Back to the projection centre for `eye` (the reference's behaviour); a focus radius stays.  Graphs captured
+ * with a focus read the projection centre from then on; once no eye has a focus or a focus radius, applies stop
+ * issuing the copy. */
 OVRFSR_API int ovrfsr_clear_focus(ovrfsr_ctx *ctx, int eye);
+/* Radius of eye's mask, in the units of ovrfsr_config::radius (R = uint(0.5 * radius * outH), host::centre_radius's
+ * truncation).  Late-latched exactly like ovrfsr_set_focus; independent of it (a radius without a focus grows or
+ * shrinks the circle around the projection centre).  For a side-by-side texture the left eye's radius applies to
+ * the left centre and the right eye's to the right one.  Stored as given, so it survives ovrfsr_reset,
+ * ovrfsr_set_config and source-size changes; a new ovrfsr_config::radius applies to eyes without one.  Lets a host
+ * widen the mask while its gaze data cannot be trusted (blink, saccade, lost tracking) without a reset.
+ * OVRFSR_ERR_INVALID for eye not in {0,1}, or radius not finite, negative or > 4 (R <= 2 * outH, so the kernels'
+ * u32 square cannot wrap for outH <= 16384); the previous value stays.  Host memory only. */
+OVRFSR_API int ovrfsr_set_focus_radius(ovrfsr_ctx *ctx, int eye, float radius);
+/* back to ovrfsr_config::radius for eye; the focus stays */
+OVRFSR_API int ovrfsr_clear_focus_radius(ovrfsr_ctx *ctx, int eye);
 
 /* ---- individual dispatches (ApplyUpscaling / ApplySharpening, PostProcessor.cpp:385-401,483-496) --
  * Stateless: explicit constant blocks, caller-owned destination.  math_mode as ovrfsr_math. */

@@ -216,6 +216,15 @@ class PostProcessor:
         """ovrfsr_clear_focus: back to the projection centre for `eye`."""
         L.check(L.lib().ovrfsr_clear_focus(self._ctx, eye), "ovrfsr_clear_focus", self._ctx)
 
+    def set_focus_radius(self, eye: int, radius: float):
+        """ovrfsr_set_focus_radius: `eye`'s radius mask uses `radius` (the units of Config.radius, in [0, 4]) instead of
+        Config.radius, with no reset.  Late-latched like set_focus and independent of it; survives set_config."""
+        L.check(L.lib().ovrfsr_set_focus_radius(self._ctx, eye, radius), "ovrfsr_set_focus_radius", self._ctx)
+
+    def clear_focus_radius(self, eye: int):
+        """ovrfsr_clear_focus_radius: back to Config.radius for `eye`."""
+        L.check(L.lib().ovrfsr_clear_focus_radius(self._ctx, eye), "ovrfsr_clear_focus_radius", self._ctx)
+
     def apply(self, eye: int, texture, bounds: TextureBounds | None = None, fmt: int | None = None, stream=None,
               samples: int = 1):
         """vr::PostProcessor::Apply.  Returns a torch tensor VIEW of the ctx-owned output (valid until the next

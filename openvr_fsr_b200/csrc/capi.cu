@@ -100,19 +100,23 @@ cudaError_t expand_rgb32f(const ovrfsr_image &src, const ovrfsr_image &dst, cuda
   return cudaGetLastError();
 }
 
-// The radius mask's focus (ovrfsr_set_focus).  `slot` (pinned host memory, one 16-byte block of imageCentre words per
-// eye) is what each apply's H2D copy reads when it runs on the GPU; it is written under `mu` only, each (x, y) pair
-// with one aligned 64-bit store, so a copy that overlaps an update sees whole pairs.  No CUDA call is made under `mu`.
+// The radius mask's focus and radius (ovrfsr_set_focus, ovrfsr_set_focus_radius).  `slot` (pinned host memory, one
+// 32-byte block per eye: imageCentre[4], radiusSq[2], two words of padding) is what each apply's H2D copy reads when it
+// runs on the GPU; it is written under `mu` only, each centre pair and the radius pair with one aligned 64-bit store,
+// so a copy that overlaps an update sees whole pairs.  No CUDA call is made under `mu`.
+constexpr int kFocusWords = 8;
 struct Focus {
   std::mutex mu;
   bool set[2] = {false, false};
   float xy[2][2] = {};
+  bool radiusSet[2] = {false, false};
+  float radius[2] = {};     // in the units of ovrfsr_config::radius
   // what the words are computed for: the ctx's config, layout and output size at its last prepare_resources
   bool ready = false;
   ovrfsr_config cfg{};
   bool onlyOneEye = true;
   uint32_t outW = 0, outH = 0;
-  uint32_t *slot = nullptr; // [2][4], allocated by the first apply that needs it
+  uint32_t *slot = nullptr; // [2][kFocusWords], allocated by the first apply that needs it
 };
 
 } // namespace
@@ -153,8 +157,9 @@ struct ovrfsr_ctx {
   // ovrfsr_apply_pair: the right eye's chain runs on this stream between a fork and a join event
   cudaStream_t pairStream = nullptr;
   cudaEvent_t pairFork = nullptr, pairJoin = nullptr;
-  // ovrfsr_set_focus: `active` once some eye has a focus; then each apply copies its eye's slot block into `focusDev`
-  // ([2][4] words, device) at its head, and the masked kernels read their centre words from there
+  // ovrfsr_set_focus / ovrfsr_set_focus_radius: `active` while some eye has a focus or a radius override; then each
+  // apply copies its eye's slot block into `focusDev` ([2][kFocusWords] words, device) at its head, and the masked
+  // kernels read their centre and radius words from there
   Focus focus;
   std::atomic<bool> focusActive{false};
   uint32_t *focusDev = nullptr;
@@ -188,43 +193,59 @@ int select_device(ovrfsr_ctx *c) {
   return OVRFSR_OK;
 }
 
-// the slot's words: host::centre_radius with each focused eye's proj_centre pair replaced by its focus (block 1 of a
-// shared texture is never read)
+// the slot's words: host::centre_radius with each focused eye's proj_centre pair replaced by its focus, and radiusSq[k]
+// the R^2 of the eye centre pair k is sourced from -- with that eye's radius override, if any, in place of cfg.radius.
+// Block e of one-eye-per-texture submits takes both words from eye e; block 0 of a shared texture takes pair 0 from the
+// left eye and pair 1 from the right (block 1 of a shared texture is never read).
 void write_focus_slot(Focus &f) {
   if (!f.slot || !f.ready) return;
   ovrfsr_config cfg = f.cfg;
   for (int e = 0; e < 2; ++e)
     if (f.set[e]) { cfg.proj_centre[2 * e] = f.xy[e][0]; cfg.proj_centre[2 * e + 1] = f.xy[e][1]; }
+  uint32_t eyeRsq[2];
+  for (int e = 0; e < 2; ++e) {
+    ovrfsr_config r = cfg;
+    if (f.radiusSet[e]) r.radius = f.radius[e];
+    uint32_t centre[4], radius[4];
+    host::centre_radius(centre, radius, r, 0, true, f.outW, f.outH); // radius[1] does not depend on the eye or layout
+    eyeRsq[e] = radius[1];
+  }
   for (int b = 0; b < 2; ++b) {
-    alignas(8) uint32_t centre[4], radius[4];
-    host::centre_radius(centre, radius, cfg, b, f.onlyOneEye, f.outW, f.outH);
-    uint64_t pair[2];
-    std::memcpy(pair, centre, sizeof(pair));
-    uint64_t *dst = reinterpret_cast<uint64_t *>(f.slot + 4 * b);
-    __atomic_store_n(&dst[0], pair[0], __ATOMIC_RELAXED);
-    __atomic_store_n(&dst[1], pair[1], __ATOMIC_RELAXED);
+    alignas(8) uint32_t words[6];
+    uint32_t radius[4];
+    host::centre_radius(words, radius, cfg, b, f.onlyOneEye, f.outW, f.outH);
+    words[4] = eyeRsq[f.onlyOneEye ? b : 0];
+    words[5] = eyeRsq[f.onlyOneEye ? b : 1];
+    uint64_t pair[3];
+    std::memcpy(pair, words, sizeof(pair));
+    uint64_t *dst = reinterpret_cast<uint64_t *>(f.slot + kFocusWords * b);
+    for (int k = 0; k < 3; ++k) __atomic_store_n(&dst[k], pair[k], __ATOMIC_RELAXED);
   }
 }
 
-// head of an apply with a focus active: copy this eye's slot block to its device block on `s`, so the kernels of the
-// apply see the focus the slot holds when the copy runs (and a captured graph re-reads the slot on every replay)
+// head of an apply with a focus or a radius override active: copy this eye's slot block to its device block on `s`, so
+// the kernels of the apply see the words the slot holds when the copy runs (and a captured graph re-reads the slot on
+// every replay)
 int latch_focus(ovrfsr_ctx *c, int eye, cudaStream_t s, const uint32_t **centreDev) {
   Focus &f = c->focus;
+  constexpr size_t kBytes = 2 * kFocusWords * sizeof(uint32_t);
   if (!f.slot) {
     uint32_t *slot = nullptr;
-    cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&slot), 2 * 4 * sizeof(uint32_t), cudaHostAllocPortable);
+    cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&slot), kBytes, cudaHostAllocPortable);
     if (e != cudaSuccess) return fail(c, OVRFSR_ERR_NOMEM, "allocating the focus slot", e);
+    std::memset(slot, 0, kBytes); // the padding words
     std::lock_guard<std::mutex> lock(f.mu);
     f.slot = slot;
     write_focus_slot(f);
   }
   if (!c->focusDev) {
-    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&c->focusDev), 2 * 4 * sizeof(uint32_t));
+    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&c->focusDev), kBytes);
     if (e != cudaSuccess) { c->focusDev = nullptr; return fail(c, OVRFSR_ERR_NOMEM, "allocating the focus block", e); }
   }
-  cudaError_t e = cudaMemcpyAsync(c->focusDev + 4 * eye, f.slot + 4 * eye, 4 * sizeof(uint32_t), cudaMemcpyHostToDevice, s);
+  cudaError_t e = cudaMemcpyAsync(c->focusDev + kFocusWords * eye, f.slot + kFocusWords * eye, kFocusWords * sizeof(uint32_t),
+                                  cudaMemcpyHostToDevice, s);
   if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "focus copy", e);
-  *centreDev = c->focusDev + 4 * eye;
+  *centreDev = c->focusDev + kFocusWords * eye;
   return OVRFSR_OK;
 }
 
@@ -306,7 +327,10 @@ void harvest_queries(ovrfsr_ctx *c) {
 }
 
 // EASU followed by RCAS in one apply with a UNORM target: EASU writes the outside-radius groups straight to the final
-// image and RCAS only visits what is inside the radius (kernels.h)
+// image and RCAS only visits what is inside the radius (kernels.h).  The two passes must classify every group the same
+// way, or a group would be written by neither or filtered twice: with a focus or a radius override both read their
+// centre and radius words from the one device block that the single copy at the head of the apply wrote on the same
+// stream (apply_post_process), so an update that lands between the two launches cannot split them.
 bool paired_passes(const ovrfsr_ctx *c) {
   static const bool off = getenv("OVRFSR_NO_PAIR") != nullptr; // dev A/B switch
   return !off && !c->cfg.use_nis && upscale_pass(c->cfg) && sharpen_pass(c->cfg) &&
@@ -642,7 +666,29 @@ int ovrfsr_clear_focus(ovrfsr_ctx *ctx, int eye) {
   std::lock_guard<std::mutex> lock(f.mu);
   f.set[eye] = false;
   write_focus_slot(f); // graphs captured with a focus fall back to the projection centre
-  ctx->focusActive.store(f.set[0] || f.set[1], std::memory_order_release);
+  ctx->focusActive.store(f.set[0] || f.set[1] || f.radiusSet[0] || f.radiusSet[1], std::memory_order_release);
+  return OVRFSR_OK;
+}
+
+int ovrfsr_set_focus_radius(ovrfsr_ctx *ctx, int eye, float radius) {
+  // 4 keeps R = 2 * outH, so R^2 <= 2^30 for outH <= 16384: the kernels' u32 square cannot wrap
+  if (!ctx || (eye != 0 && eye != 1) || !(radius >= 0.f && radius <= 4.f)) return OVRFSR_ERR_INVALID;
+  Focus &f = ctx->focus;
+  std::lock_guard<std::mutex> lock(f.mu);
+  f.radiusSet[eye] = true;
+  f.radius[eye] = radius;
+  write_focus_slot(f);
+  ctx->focusActive.store(true, std::memory_order_release);
+  return OVRFSR_OK;
+}
+
+int ovrfsr_clear_focus_radius(ovrfsr_ctx *ctx, int eye) {
+  if (!ctx || (eye != 0 && eye != 1)) return OVRFSR_ERR_INVALID;
+  Focus &f = ctx->focus;
+  std::lock_guard<std::mutex> lock(f.mu);
+  f.radiusSet[eye] = false;
+  write_focus_slot(f); // graphs captured with an override fall back to ovrfsr_config::radius
+  ctx->focusActive.store(f.set[0] || f.set[1] || f.radiusSet[0] || f.radiusSet[1], std::memory_order_release);
   return OVRFSR_OK;
 }
 

@@ -37,7 +37,7 @@ struct FusedArgs {
   ImageRW dst;
   float c0x, c0y, c0z, c0w;
   uint32_t centre[4];
-  const uint32_t *centreDev; // nullptr: `centre`; else the device block holding the imageCentre words (load_centre)
+  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`; else the device block holding the mask words (load_centre)
   uint32_t radiusSq;
   float radW, radH;
   int tileW, tileH;   // shared source tile extent in texels (for the 66 x 34 region)
@@ -90,8 +90,8 @@ __global__ void __launch_bounds__(kThreads, 2) fsr_fused_kernel(const __grid_con
     __syncthreads();
   }
 
-  uint32_t centre[4];
-  load_centre(centre, a.centre, a.centreDev);
+  uint32_t centre[4], rsq[2];
+  load_centre(centre, rsq, a.centre, a.radiusSq, a.centreDev);
   uint32_t phase = 0;
   for (; t < numTiles; t += gridDim.x) {
     int ox0, oy0, sx0, sy0;
@@ -104,7 +104,7 @@ __global__ void __launch_bounds__(kThreads, 2) fsr_fused_kernel(const __grid_con
     // image only hold out-of-image pixels, whose class is never used)
     if (warp == 0) {
       const uint32_t ggx = (uint32_t)(ox0 >> 4) - 1u + (uint32_t)(lane % 6), ggy = (uint32_t)(oy0 >> 4) - 1u + (uint32_t)(lane / 6);
-      const bool in = lane < 24 && group_inside(ggx * 16u + 8u, ggy * 16u + 8u, centre, a.radiusSq);
+      const bool in = lane < 24 && group_inside(ggx * 16u + 8u, ggy * 16u + 8u, centre, rsq[0], rsq[1]);
       const uint32_t m = __ballot_sync(0xffffffffu, in);
       if (lane == 0) sGroupMask = m;
     }

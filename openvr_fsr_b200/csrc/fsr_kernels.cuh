@@ -32,7 +32,7 @@ struct EasuArgs {
   ImageRW dst;
   float c0x, c0y, c0z, c0w; // const0 of FsrEasuCon: out->in scale and offset
   uint32_t centre[4];
-  const uint32_t *centreDev; // nullptr: `centre`; else the device block holding the imageCentre words (load_centre)
+  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`; else the device block holding the mask words (load_centre)
   uint32_t radiusSq;
   float radW, radH;         // (float)Radius.z, (float)Radius.w for Bilinear()
   int tileW, tileH;         // shared source tile extent in texels
@@ -50,7 +50,7 @@ struct RcasArgs {
   float sharp;              // const0[0] as float
   float tintGB;             // 1 - debug*0.3 (fsr_rcas.hlsl:46)
   uint32_t centre[4];
-  const uint32_t *centreDev; // nullptr: `centre`; else the device block holding the imageCentre words (load_centre)
+  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`; else the device block holding the mask words (load_centre)
   uint32_t radiusSq;
   int skipOutside;          // the preceding EASU launch already wrote the outside-radius groups to dst (EasuArgs::direct)
   int opaqueSrc;            // B8G8R8X8 source: the X byte reads as alpha 1 (only the outside-radius copy looks at alpha)
@@ -444,16 +444,16 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
 
   // this warp's 16x16 group and its radius test (warp-uniform)
   const uint32_t ggx = (uint32_t)(ox0 >> 4) + (warp & 3), ggy = (uint32_t)(oy0 >> 4) + (warp >> 2);
-  uint32_t centre[4];
-  load_centre(centre, a.centre, a.centreDev);
-  const bool inside = group_inside(ggx * 16u + 8u, ggy * 16u + 8u, centre, a.radiusSq);
+  uint32_t centre[4], rsq[2];
+  load_centre(centre, rsq, a.centre, a.radiusSq, a.centreDev);
+  const bool inside = group_inside(ggx * 16u + 8u, ggy * 16u + 8u, centre, rsq[0], rsq[1]);
   constexpr bool direct = PAIRED && (FOUT == OVRFSR_FORMAT_RGBA8 || FOUT == OVRFSR_FORMAT_RGB10A2);
   // outside group, paired: the intermediate is still needed where RCAS of an edge-adjacent inside group reads across
-  // the group edge (tested here so that the centre words need not stay live through the filter)
-  const bool mid = !direct || inside || group_inside(ggx * 16u - 8u, ggy * 16u + 8u, centre, a.radiusSq) ||
-                   group_inside(ggx * 16u + 24u, ggy * 16u + 8u, centre, a.radiusSq) ||
-                   group_inside(ggx * 16u + 8u, ggy * 16u - 8u, centre, a.radiusSq) ||
-                   group_inside(ggx * 16u + 8u, ggy * 16u + 24u, centre, a.radiusSq);
+  // the group edge (tested here so that the mask words need not stay live through the filter)
+  const bool mid = !direct || inside || group_inside(ggx * 16u - 8u, ggy * 16u + 8u, centre, rsq[0], rsq[1]) ||
+                   group_inside(ggx * 16u + 24u, ggy * 16u + 8u, centre, rsq[0], rsq[1]) ||
+                   group_inside(ggx * 16u + 8u, ggy * 16u - 8u, centre, rsq[0], rsq[1]) ||
+                   group_inside(ggx * 16u + 8u, ggy * 16u + 24u, centre, rsq[0], rsq[1]);
 
   // ---- stage 1: decode the clamped source tile once, loads batched per thread for ILP -------------
   if constexpr (TMA) {
@@ -752,14 +752,14 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
   // same UNORM layout in and out: outside-radius texels pass through bit for bit
   constexpr bool kRawCopy = FIN == FOUT && (FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_RGB10A2);
 
-  uint32_t centre[4];
-  load_centre(centre, a.centre, a.centreDev);
+  uint32_t centre[4], rsq[2];
+  load_centre(centre, rsq, a.centre, a.radiusSq, a.centreDev);
   if constexpr (PAIRED) {
     // uniform per CTA: nothing of this tile is inside the radius -> nothing to do (and no TMA load is issued)
     bool any = false;
 #pragma unroll
     for (int g = 0; g < 8; ++g)
-      any = any || group_inside((blockIdx.x * 4u + (g & 3)) * 16u + 8u, (blockIdx.y * 2u + (g >> 2)) * 16u + 8u, centre, a.radiusSq);
+      any = any || group_inside((blockIdx.x * 4u + (g & 3)) * 16u + 8u, (blockIdx.y * 2u + (g >> 2)) * 16u + 8u, centre, rsq[0], rsq[1]);
     if (!any) return;
   }
   if constexpr (TMA) {
@@ -771,7 +771,7 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
     }
   }
   const uint32_t ggx = blockIdx.x * (kTileW / 16) + (warp & 3), ggy = blockIdx.y * (kTileH / 16) + (warp >> 2);
-  const bool inside = group_inside(ggx * 16u + 8u, ggy * 16u + 8u, centre, a.radiusSq);
+  const bool inside = group_inside(ggx * 16u + 8u, ggy * 16u + 8u, centre, rsq[0], rsq[1]);
 
   if constexpr (TMA) {
     // a CTA whose 8 groups are all outside the radius and copy raw bytes needs no decoded tile at all

@@ -17,8 +17,9 @@ struct PassImage { void *ptr; uint32_t pitch; int w, h; int format; bool array =
 // apply, EASU writes the outside-radius groups -- which RCAS would only copy (x the debug tint `tintGB`) -- straight
 // to the final image `direct`, and RCAS visits only tiles / groups inside the radius.  Same output bits as two plain
 // dispatches; a stateless dispatch passes nullptr / false.
-// `centreDev` (every masked launcher): nullptr = the imageCentre words of the constant block; else a 16-byte device block
-// the kernels read those four words from when they run (the ctx path with a focus, ovrfsr_set_focus).
+// `centreDev` (every masked launcher): nullptr = the imageCentre and radiusSq words of the constant block; else a 32-byte
+// device block {imageCentre[4], radiusSq[2], pad[2]} the kernels read those words from when they run (the ctx path with
+// a focus or a focus radius, ovrfsr_set_focus / ovrfsr_set_focus_radius); radiusSq[k] is centre pair k's squared radius.
 // `srtm` (EASU and RCAS): OVRFSR_PASS_SRTM_* bits, AMD's reversible tone map on the texels read / the pixels stored.
 // Float sources only, and never together with the pairing: cudaErrorInvalidValue otherwise.
 cudaError_t launch_easu_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,

@@ -145,4 +145,15 @@ bool PostProcessor::ClearFocus(EVREye eEye) {
   return c && ovrfsr_clear_focus(c, eEye == Eye_Right ? 1 : 0) == OVRFSR_OK;
 }
 
+// like the focus, the radius override lives in the ctx and survives the set_config of the first Apply and every Reset
+bool PostProcessor::SetFocusRadius(EVREye eEye, float radius) {
+  ovrfsr_ctx *c = Context();
+  return c && ovrfsr_set_focus_radius(c, eEye == Eye_Right ? 1 : 0, radius) == OVRFSR_OK;
+}
+
+bool PostProcessor::ClearFocusRadius(EVREye eEye) {
+  ovrfsr_ctx *c = Context();
+  return c && ovrfsr_clear_focus_radius(c, eEye == Eye_Right ? 1 : 0) == OVRFSR_OK;
+}
+
 } // namespace vr

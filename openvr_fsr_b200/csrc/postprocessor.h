@@ -49,6 +49,12 @@ public:
   // (x / y not finite or outside [0, 1]).
   bool SetFocus(EVREye eEye, float x, float y);
   bool ClearFocus(EVREye eEye);
+  // Dynamic foveation (ovrfsr_set_focus_radius / ovrfsr_clear_focus_radius): the radius mask of `eEye` uses `radius`
+  // (the units of Config::radius) instead of Config::radius, from the next frame whose GPU work starts after the
+  // call, with no Reset -- e.g. widened while the tracker's sample for that eye is invalid.  Same threading as
+  // SetFocus.  false: rejected (radius not finite, negative or > 4).
+  bool SetFocusRadius(EVREye eEye, float radius);
+  bool ClearFocusRadius(EVREye eEye);
 
 private:
   ovrfsr_ctx *Context(); // creates the ctx on first use (no GPU work); guarded by ctxMutex
