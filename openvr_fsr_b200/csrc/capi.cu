@@ -4,7 +4,6 @@
 // calls fail with OVRFSR_ERR_CUDA.
 #include <atomic>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <new>
@@ -40,6 +39,10 @@ struct DeviceImage {
     img.width = w; img.height = h; img.format = fmt; img.array_slices = 1; img.slice_pitch = 0;
     img.pitch = align_up(w * bytes_per_pixel(fmt), 256u);
     return cudaMalloc(&img.data, (size_t)img.pitch * h) == cudaSuccess;
+  }
+  // keep the image if it has this size and format, else reallocate it
+  bool ensure(uint32_t w, uint32_t h, int fmt) {
+    return (img.data && img.width == w && img.height == h && img.format == fmt) || alloc(w, h, fmt);
   }
   void release() {
     if (img.data) cudaFree(img.data);
@@ -119,6 +122,24 @@ struct Focus {
   uint32_t *slot = nullptr; // [2][kFocusWords], allocated by the first apply that needs it
 };
 
+// What every apply of a context runs (PostProcessor.cpp:586-594), decided by prepare_resources from the config, the
+// source format and the output format, none of which can change before the next prepare_resources.  FSR always runs
+// RCAS, after EASU when upscaling; NIS runs one pass, NVScaler when upscaling and NVSharpen otherwise.  The last pass
+// writes the caller's image or the ctx's output image.
+struct Plan {
+  bool nis = false;
+  bool upscale = false; // render_scale != 1
+  // EASU followed by RCAS with a UNORM target: EASU writes the outside-radius groups straight to the final image and
+  // RCAS only visits what is inside the radius (kernels.h).  The two passes must classify every group the same way, or
+  // a group would be written by neither or filtered twice: with a focus or a radius override both read their centre
+  // and radius words from the one device block that the single copy at the head of the apply wrote on the same stream
+  // (apply_post_process), so an update that lands between the two launches cannot split them.
+  bool paired = false;
+  bool tryFused = false;          // paired and OVRFSR_FLAG_FUSED_FSR: one fused kernel, where the images allow it
+  int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* of each FSR pass
+  int midFormat = OVRFSR_FORMAT_RGBA8; // of FSR's upscaled image
+};
+
 } // namespace
 
 struct ovrfsr_ctx {
@@ -135,8 +156,10 @@ struct ovrfsr_ctx {
   uint32_t sharpenConstants[2][12]{};
   alignas(16) uint8_t nisScalerConfig[2][256]{};
   alignas(16) uint8_t nisSharpenConfig[2][256]{};
-  // one set of intermediates/outputs PER EYE (the reference shares one; see ovrfsr.h)
-  DeviceImage upscaled[2], sharpened[2];
+  Plan plan;
+  // one set of intermediates/outputs PER EYE (the reference shares one; see ovrfsr.h): FSR's upscaled image, and the
+  // image the last pass writes when the caller passes none
+  DeviceImage upscaled[2], output[2];
   DeviceImage hostStage[2]; // device staging of host-submitted eyes (ovrfsr_apply_host)
   DeviceBuffer hostLinearIn[2], hostLinearOut[2];
   DeviceImage resolved[2];  // copiedTexture (PostProcessor.h:29): the resolved copy of a multisampled source
@@ -177,7 +200,7 @@ int fail(ovrfsr_ctx *ctx, int status, const char *what, cudaError_t e = cudaSucc
 }
 
 void release_resources(ovrfsr_ctx *c) {
-  for (int e = 0; e < 2; ++e) { c->upscaled[e].release(); c->sharpened[e].release(); c->hostStage[e].release(); c->hostLinearIn[e].release(); c->hostLinearOut[e].release(); c->resolved[e].release(); c->expanded[e].release(); }
+  for (int e = 0; e < 2; ++e) { c->upscaled[e].release(); c->output[e].release(); c->hostStage[e].release(); c->hostLinearIn[e].release(); c->hostLinearOut[e].release(); c->resolved[e].release(); c->expanded[e].release(); }
   if (c->focusDev) { cudaFree(c->focusDev); c->focusDev = nullptr; }
   if (c->evCreated) {
     for (int i = 0; i < kQueryCount; ++i) { cudaEventDestroy(c->evStart[i]); cudaEventDestroy(c->evEnd[i]); c->evPending[i] = false; }
@@ -249,21 +272,6 @@ int latch_focus(ovrfsr_ctx *c, int eye, cudaStream_t s, const uint32_t **centreD
   return OVRFSR_OK;
 }
 
-bool upscale_pass(const ovrfsr_config &cfg) { return cfg.render_scale != 1.f; }                    // PostProcessor.cpp:586
-bool sharpen_pass(const ovrfsr_config &cfg) { return !cfg.use_nis || cfg.render_scale == 1.f; }    // PostProcessor.cpp:591
-// both FSR passes run and the caller opted into the fused kernel (the intermediate is then never materialised)
-// OVRFSR_FLAG_SRTM takes effect on the FSR path with a float source (an RGB32F one is read through its RGBA32F copy, a
-// multisampled one after its resolve); UNORM sources are display-referred already and NIS has HDR modes of its own
-bool srtm_source(int fmt) { return fmt == OVRFSR_FORMAT_RGBA16F || fmt == OVRFSR_FORMAT_RGBA32F || fmt == OVRFSR_FORMAT_RGB32F; }
-bool srtm_pass(const ovrfsr_config &cfg, int inFormat) { return (cfg.flags & OVRFSR_FLAG_SRTM) && !cfg.use_nis && srtm_source(inFormat); }
-bool fused_pass(const ovrfsr_config &cfg, int inFormat) {
-  return !cfg.use_nis && upscale_pass(cfg) && sharpen_pass(cfg) && (cfg.flags & OVRFSR_FLAG_FUSED_FSR) && !srtm_pass(cfg, inFormat);
-}
-// Format of the upscaled image.  The reference's rule is the output format; with SRTM, EASU stores tone-mapped values
-// that RCAS's G amplifies by up to 32768 near 1, so the intermediate keeps them as RGBA32F for a float output, and as
-// RGBA16F for a UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).
-int mid_format(const ovrfsr_ctx *c);
-
 // PostProcessor::PrepareResources, PostProcessor.cpp:498-561
 int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
   c->inputWidth = src->width;
@@ -279,6 +287,24 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
       c->outFormat != (tenBit ? OVRFSR_FORMAT_RGB10A2 : OVRFSR_FORMAT_RGBA8))
     return fail(c, OVRFSR_ERR_UNSUPPORTED, tenBit ? "output format for an RGB10A2 source must be RGB10A2, RGBA16F or RGBA32F"
                                                   : "output format must be RGBA8, RGBA16F or RGBA32F");
+  Plan &p = c->plan;
+  p.nis = c->cfg.use_nis != 0;
+  p.upscale = c->cfg.render_scale != 1.f;
+  const bool unormOut = c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2;
+  // OVRFSR_FLAG_SRTM takes effect on the FSR path with a float source (an RGB32F one is read through its RGBA32F copy, a
+  // multisampled one after its resolve); UNORM sources are display-referred already and NIS has HDR modes of its own
+  const bool srtm = !p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM) &&
+                    (src->format == OVRFSR_FORMAT_RGBA16F || src->format == OVRFSR_FORMAT_RGBA32F || src->format == OVRFSR_FORMAT_RGB32F);
+  p.paired = !p.nis && p.upscale && unormOut && !srtm;
+  p.tryFused = p.paired && (c->cfg.flags & OVRFSR_FLAG_FUSED_FSR);
+  // SRTM: EASU applies F on read and stores tone-mapped values, RCAS applies G on store, and F on read too when it is
+  // the only pass
+  p.easuSrtm = srtm ? OVRFSR_PASS_SRTM_IN : 0;
+  p.rcasSrtm = !srtm ? 0 : OVRFSR_PASS_SRTM_OUT | (p.upscale ? 0 : OVRFSR_PASS_SRTM_IN);
+  // The reference's upscaled image has the output format; with SRTM, EASU stores tone-mapped values that RCAS's G
+  // amplifies by up to 32768 near 1, so the intermediate keeps them as RGBA32F for a float output, and as RGBA16F for a
+  // UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).
+  p.midFormat = !srtm ? c->outFormat : (unormOut ? OVRFSR_FORMAT_RGBA16F : OVRFSR_FORMAT_RGBA32F);
   const bool one = c->textureContainsOnlyOneEye;
   const int neyes = one ? 2 : 1;
   for (int e = 0; e < neyes; ++e) {
@@ -289,13 +315,13 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
                            c->outputHeight);
     ovrfsr_make_nis_config(c->nisSharpenConfig[e], &c->cfg, 1, e, one, c->inputWidth, c->inputHeight, c->outputWidth,
                            c->outputHeight);
-    // the upscaled image only exists when the two dispatches run (the fused kernel keeps it in shared memory; if a
-    // shape turns out not to be fusable it is allocated on first use)
-    const bool wantMid = upscale_pass(c->cfg) && !(fused_pass(c->cfg, c->inFormat) && (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2));
-    if (wantMid && !c->upscaled[e].alloc(c->outputWidth, c->outputHeight, mid_format(c)))
+    // the upscaled image only exists when EASU and RCAS run as two dispatches (the fused kernel keeps it in shared
+    // memory; if a shape turns out not to be fusable it is allocated on first use)
+    if (!p.nis && p.upscale && !p.tryFused && !c->upscaled[e].alloc(c->outputWidth, c->outputHeight, p.midFormat))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
-    if (sharpen_pass(c->cfg) && !c->sharpened[e].alloc(c->outputWidth, c->outputHeight, c->outFormat))
-      return fail(c, OVRFSR_ERR_NOMEM, "allocating sharpened texture", cudaGetLastError());
+    if (!c->output[e].alloc(c->outputWidth, c->outputHeight, c->outFormat))
+      return fail(c, OVRFSR_ERR_NOMEM, p.nis && p.upscale ? "allocating upscaled texture" : "allocating sharpened texture",
+                  cudaGetLastError());
   }
   if (c->cfg.debug_mode) {
     for (int i = 0; i < kQueryCount; ++i) {
@@ -324,61 +350,6 @@ void harvest_queries(ovrfsr_ctx *c) {
     if (cudaEventElapsedTime(&ms, c->evStart[i], c->evEnd[i]) == cudaSuccess) { c->summedGpuTime += ms; ++c->countedQueries; }
     c->evPending[i] = false;
   }
-}
-
-// EASU followed by RCAS in one apply with a UNORM target: EASU writes the outside-radius groups straight to the final
-// image and RCAS only visits what is inside the radius (kernels.h).  The two passes must classify every group the same
-// way, or a group would be written by neither or filtered twice: with a focus or a radius override both read their
-// centre and radius words from the one device block that the single copy at the head of the apply wrote on the same
-// stream (apply_post_process), so an update that lands between the two launches cannot split them.
-bool paired_passes(const ovrfsr_ctx *c) {
-  static const bool off = getenv("OVRFSR_NO_PAIR") != nullptr; // dev A/B switch
-  return !off && !c->cfg.use_nis && upscale_pass(c->cfg) && sharpen_pass(c->cfg) &&
-         (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2) && !srtm_pass(c->cfg, c->inFormat);
-}
-
-int mid_format(const ovrfsr_ctx *c) {
-  if (!srtm_pass(c->cfg, c->inFormat) || !sharpen_pass(c->cfg)) return c->outFormat;
-  return (c->outFormat == OVRFSR_FORMAT_RGBA16F || c->outFormat == OVRFSR_FORMAT_RGBA32F) ? OVRFSR_FORMAT_RGBA32F : OVRFSR_FORMAT_RGBA16F;
-}
-
-int nis_status(cudaError_t e) {
-  return (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA;
-}
-
-// fin: the image the apply's last pass writes (EASU's outside-radius groups go there when RCAS follows); centreDev: the
-// focus block latched for this apply, or nullptr
-int run_upscale(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &out, const PassImage &fin, cudaStream_t s,
-                const uint32_t *centreDev) {
-  const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
-  cudaError_t e;
-  if (c->cfg.use_nis) {
-    e = launch_nis(false, in, out, c->nisScalerConfig[eye], c->cfg.math_mode, s, centreDev);
-    return e == cudaSuccess ? OVRFSR_OK : fail(c, nis_status(e), "NIS scaler dispatch", e);
-  }
-  const PassImage *direct = paired_passes(c) ? &fin : nullptr;
-  const float tint = 1.0f - (float)c->sharpenConstants[eye][3] * 0.3f;
-  // SRTM: F on read; the tone-mapped result goes to the intermediate and RCAS maps it back (RCAS always follows EASU
-  // on the FSR path)
-  const int srtm = srtm_pass(c->cfg, c->inFormat) ? OVRFSR_PASS_SRTM_IN : 0;
-  e = strict ? launch_easu_strict(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev, srtm)
-             : launch_easu_fast(in, out, c->upscaleConstants[eye], s, direct, tint, centreDev, srtm);
-  return e == cudaSuccess ? OVRFSR_OK : fail(c, OVRFSR_ERR_CUDA, "EASU launch", e);
-}
-
-int run_sharpen(ovrfsr_ctx *c, int eye, const PassImage &in, const PassImage &out, cudaStream_t s, const uint32_t *centreDev) {
-  const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
-  if (c->cfg.use_nis) {
-    const cudaError_t e = launch_nis(true, in, out, c->nisSharpenConfig[eye], c->cfg.math_mode, s, centreDev);
-    return e == cudaSuccess ? OVRFSR_OK : fail(c, nis_status(e), "NIS sharpen dispatch", e);
-  }
-  const bool skip = paired_passes(c);
-  // SRTM: G on store; F on read too when RCAS is the only pass (after EASU its source is tone-mapped already)
-  const int srtm = !srtm_pass(c->cfg, c->inFormat) ? 0
-                   : OVRFSR_PASS_SRTM_OUT | (upscale_pass(c->cfg) ? 0 : OVRFSR_PASS_SRTM_IN);
-  cudaError_t e = strict ? launch_rcas_strict(in, out, c->sharpenConstants[eye], s, skip, centreDev, srtm)
-                         : launch_rcas_fast(in, out, c->sharpenConstants[eye], s, skip, centreDev, srtm);
-  return e == cudaSuccess ? OVRFSR_OK : fail(c, OVRFSR_ERR_CUDA, "RCAS launch", e);
 }
 
 // PostProcessor::SaveTextureToFile, PostProcessor.cpp:640-657: staging copy, then the DDS writer (capture.cpp)
@@ -412,28 +383,25 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
   // GetInputView: array textures keep the right eye in slice 1 (PostProcessor.cpp:254-268)
   const int slice = (src->array_slices > 1 && eye == 1) ? 1 : 0;
   PassImage in = pass_image(*src, slice);
-  Image result = *src;
+  cudaError_t e;
   if (src->sample_count > 1) { // GetInputView: multisampled sources are resolved into copiedTexture first (:219-226)
     DeviceImage &r = c->resolved[eye];
-    if ((!r.img.data || r.img.width != src->width || r.img.height != src->height || r.img.format != src->format) &&
-        !r.alloc(src->width, src->height, src->format))
+    if (!r.ensure(src->width, src->height, src->format))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating the MSAA resolve target", cudaGetLastError());
-    cudaError_t e = launch_resolve_msaa(in, (int)src->sample_count, pass_image(r.img), s);
+    e = launch_resolve_msaa(in, (int)src->sample_count, pass_image(r.img), s);
     if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "MSAA resolve launch", e);
     in = pass_image(r.img);
-    result = r.img;
   }
   if (src->format == OVRFSR_FORMAT_RGB32F) { // three-component float source: the kernels read it through an RGBA32F copy
     if (src->sample_count > 1) return fail(c, OVRFSR_ERR_UNSUPPORTED, "multisampled R32G32B32_FLOAT source");
     DeviceImage &x = c->expanded[eye];
-    if ((!x.img.data || x.img.width != src->width || x.img.height != src->height) && !x.alloc(src->width, src->height, OVRFSR_FORMAT_RGBA32F))
+    if (!x.ensure(src->width, src->height, OVRFSR_FORMAT_RGBA32F))
       return fail(c, OVRFSR_ERR_NOMEM, "allocating the RGBA32F copy of an RGB32F source", cudaGetLastError());
     ovrfsr_image sl = *src;
     sl.data = static_cast<uint8_t *>(src->data) + (size_t)slice * src->slice_pitch;
-    cudaError_t e = expand_rgb32f(sl, x.img, s);
+    e = expand_rgb32f(sl, x.img, s);
     if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "RGB32F expansion launch", e);
     in = pass_image(x.img);
-    result = x.img;
   }
   int q = -1;
   if (c->evCreated) {
@@ -443,41 +411,46 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
     if (c->evPending[q]) q = -1; // oldest sample still in flight: skip this frame rather than block
     else cudaEventRecord(c->evStart[q], s);
   }
-  // the sharpened image, where sharpening runs (PostProcessor.cpp:591)
-  const Image &fin = dst ? *dst : c->sharpened[eye].img;
+  // ApplyUpscaling and ApplySharpening (PostProcessor.cpp:586-594); the last pass writes fin
+  const Plan &p = c->plan;
+  const Image &fin = dst ? *dst : c->output[eye].img;
+  const PassImage finPass = pass_image(fin);
+  const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
   bool fused = false;
   // the fused kernel has no array I/O: with an array source or destination the two dispatches run
-  if (fused_pass(c->cfg, c->inFormat) && (c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2) && !src->array && !fin.array) {
-    // ApplyUpscaling + ApplySharpening (PostProcessor.cpp:586-594) as one kernel; shapes it does not cover take the
-    // two dispatches below
-    const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
-    const PassImage out2 = pass_image(fin);
-    const cudaError_t e = strict ? launch_fsr_fused_strict(in, out2, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev)
-                                 : launch_fsr_fused_fast(in, out2, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev);
-    if (e == cudaSuccess) { fused = true; result = fin; }
+  if (p.tryFused && !src->array && !fin.array) {
+    // EASU and RCAS as one kernel; shapes it does not cover take the two dispatches below
+    e = strict ? launch_fsr_fused_strict(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev)
+               : launch_fsr_fused_fast(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev);
+    if (e == cudaSuccess) fused = true;
     else if (e != cudaErrorInvalidValue && e != cudaErrorInvalidConfiguration) return fail(c, OVRFSR_ERR_CUDA, "fused EASU+RCAS launch", e);
   }
-  if (!fused && upscale_pass(c->cfg)) {
-    // without a sharpening pass the upscaled image is the output
-    const bool last = !sharpen_pass(c->cfg);
-    if (!(last && dst) && !c->upscaled[eye].img.data && !c->upscaled[eye].alloc(c->outputWidth, c->outputHeight, mid_format(c)))
-      return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
-    const Image &up = last && dst ? *dst : c->upscaled[eye].img;
-    int rc = run_upscale(c, eye, in, pass_image(up), pass_image(fin), s, centreDev);
-    if (rc != OVRFSR_OK) return rc;
-    in = pass_image(up);
-    result = up;
-  }
-  if (!fused && sharpen_pass(c->cfg)) {
-    int rc = run_sharpen(c, eye, in, pass_image(fin), s, centreDev);
-    if (rc != OVRFSR_OK) return rc;
-    result = fin;
+  if (p.nis) {
+    e = launch_nis(!p.upscale, in, finPass, p.upscale ? c->nisScalerConfig[eye] : c->nisSharpenConfig[eye], c->cfg.math_mode, s, centreDev);
+    if (e != cudaSuccess)
+      return fail(c, (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA,
+                  p.upscale ? "NIS scaler dispatch" : "NIS sharpen dispatch", e);
+  } else if (!fused) {
+    if (p.upscale) { // paired: EASU writes its outside-radius groups to fin, and RCAS skips them
+      DeviceImage &up = c->upscaled[eye];
+      if (!up.ensure(c->outputWidth, c->outputHeight, p.midFormat))
+        return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
+      const PassImage *direct = p.paired ? &finPass : nullptr;
+      const float tint = 1.0f - (float)c->sharpenConstants[eye][3] * 0.3f;
+      e = strict ? launch_easu_strict(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuSrtm)
+                 : launch_easu_fast(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuSrtm);
+      if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "EASU launch", e);
+      in = pass_image(up.img);
+    }
+    e = strict ? launch_rcas_strict(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasSrtm)
+               : launch_rcas_fast(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasSrtm);
+    if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "RCAS launch", e);
   }
   if (q >= 0) { cudaEventRecord(c->evEnd[q], s); c->evPending[q] = true; }
-  *out = result;
+  *out = fin;
   if (c->takeCapture && eye == 0) { // PostProcessor.cpp:634-637
     c->takeCapture = false;
-    int rc = save_capture(c, result, s);
+    int rc = save_capture(c, fin, s);
     if (rc != OVRFSR_OK) return rc;
   }
   return OVRFSR_OK;
@@ -500,6 +473,11 @@ int validate_image(const Image *im, bool dst = false) {
   return validate_image(static_cast<const ovrfsr_image *>(im));
 }
 
+// "Texture size changed, recreating resources" (PostProcessor.cpp:139-142); a format change does the same
+void reset_if_source_changed(ovrfsr_ctx *c, const ovrfsr_image &src) {
+  if (c->initialized && (src.width != c->inputWidth || src.height != c->inputHeight || src.format != c->inFormat)) ovrfsr_reset(c);
+}
+
 // ovrfsr_apply / ovrfsr_apply_into.  out: receives the output image (may be null); dst: the caller's output image (may
 // be null)
 int apply_impl(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *src_tagged, int only_one_eye, ovrfsr_image *out,
@@ -517,9 +495,7 @@ int apply_impl(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *src_tagged, int onl
   if ((rc = validate_image(src)) != OVRFSR_OK) return fail(ctx, rc, "invalid source image");
   if (dst && (rc = validate_image(dst, true)) != OVRFSR_OK) return fail(ctx, rc, "invalid destination image");
   if ((rc = select_device(ctx)) != OVRFSR_OK) return rc;
-  if (ctx->initialized && (src->width != ctx->inputWidth || src->height != ctx->inputHeight || src->format != ctx->inFormat)) {
-    ovrfsr_reset(ctx); // "Texture size changed, recreating resources", PostProcessor.cpp:139-142
-  }
+  reset_if_source_changed(ctx, *src);
   if (!ctx->initialized) {
     ctx->textureContainsOnlyOneEye = only_one_eye != 0; // PostProcessor.cpp:146
     rc = prepare_resources(ctx, src);
@@ -734,15 +710,12 @@ int ovrfsr_apply_host(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *src_tagged, 
   if (src_host->sample_count > 1 || dst_host->sample_count > 1) return fail(ctx, OVRFSR_ERR_UNSUPPORTED, "multisampled host images");
   if ((rc = select_device(ctx)) != OVRFSR_OK) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  // "Texture size changed, recreating resources" (PostProcessor.cpp:139-142) must happen BEFORE this eye is staged:
-  // the reset releases every ctx-owned image, the staging images included
-  if (ctx->initialized && (src_host->width != ctx->inputWidth || src_host->height != ctx->inputHeight || src_host->format != ctx->inFormat))
-    ovrfsr_reset(ctx);
+  // "Texture size changed, recreating resources" must happen BEFORE this eye is staged: the reset releases every
+  // ctx-owned image, the staging images included
+  reset_if_source_changed(ctx, *src_host);
   DeviceImage &st = ctx->hostStage[eye];
-  if (!st.img.data || st.img.width != src_host->width || st.img.height != src_host->height || st.img.format != src_host->format) {
-    if (!st.alloc(src_host->width, src_host->height, src_host->format))
-      return fail(ctx, OVRFSR_ERR_NOMEM, "allocating host staging image", cudaGetLastError());
-  }
+  if (!st.ensure(src_host->width, src_host->height, src_host->format))
+    return fail(ctx, OVRFSR_ERR_NOMEM, "allocating host staging image", cudaGetLastError());
   const size_t rowBytes = (size_t)src_host->width * bytes_per_pixel(src_host->format);
   cudaError_t e;
   if (src_host->pitch == rowBytes) { // tight host rows: one contiguous PCIe copy, re-pitched on the device
