@@ -167,7 +167,8 @@ OVRFSR_API int ovrfsr_create(ovrfsr_ctx **out, const ovrfsr_config *cfg);
 OVRFSR_API void ovrfsr_destroy(ovrfsr_ctx *ctx);
 /* PostProcessor::Reset (PostProcessor.cpp:166-194): drops every cached resource, re-enables. */
 OVRFSR_API int ovrfsr_reset(ovrfsr_ctx *ctx);
-/* What the hotkeys do (PostProcessor.cpp:670-704): mutate Config, then Reset. */
+/* What the hotkeys do (PostProcessor.cpp:670-704): mutate Config, then Reset -- on any change, sharpness included.
+ * A host that changes the sharpness while the game runs calls ovrfsr_set_sharpness instead, which needs no reset. */
 OVRFSR_API int ovrfsr_set_config(ovrfsr_ctx *ctx, const ovrfsr_config *cfg);
 OVRFSR_API int ovrfsr_get_config(const ovrfsr_ctx *ctx, ovrfsr_config *cfg);
 
@@ -221,13 +222,16 @@ OVRFSR_API int ovrfsr_apply_pair_into(ovrfsr_ctx *ctx, const ovrfsr_image *src_l
  * eye's projection centre in the imageCentre words; the radius is unchanged.  No reset, no reallocation.
  * May be called from any thread, concurrently with the ctx's apply calls.  OVRFSR_ERR_INVALID for
  * eye not in {0,1} or x/y not finite or outside [0,1].
- * Late-latched: while some eye has a focus or a focus radius (below), each apply (every ovrfsr_apply* entry)
- * starts with a 32-byte host->device copy of its eye's mask words (imageCentre[4], the squared radius of each
- * centre pair, two words of padding) on its stream, and the masked kernels read them from device memory, so a
- * frame uses the focus set before that copy RUNS; a captured CUDA graph follows later calls on every replay.
- * Each (x, y) pair, and the pair of radius words, is published with one 64-bit store: a copy that overlaps an
- * update may combine the centre pairs of one update with the radius words of another, each of them whole --
- * never the x of one update with the y of another -- and every such combination is a valid set of mask words.
+ * Late-latched: while some eye has a focus or a focus radius, or the sharpness is overridden (below), each apply
+ * (every ovrfsr_apply* entry) starts with a 64-byte host->device copy of its eye's block on its stream -- the mask
+ * words (imageCentre[4], the squared radius of each centre pair), RCAS's const0[0], the four sharpness words of the
+ * NISConfig and padding -- and the kernels read them from device memory, so a frame uses the focus set before that
+ * copy RUNS; a captured CUDA graph follows later calls on every replay.
+ * Each (x, y) pair, the pair of radius words, the NIS strength pair (kSharpStrengthMin / Scale) and the NIS limit
+ * pair (kSharpLimitMin / Scale) is published with one 64-bit store: a copy that overlaps an update may combine the
+ * centre pairs of one update with the radius words of another, or the strength pair of one sharpness update with
+ * the limit pair of another, each of them whole -- never the x of one update with the y of another -- and every
+ * such combination is a valid set of words.  RCAS's sharpness is one word and cannot tear.
  * The focus survives ovrfsr_reset, ovrfsr_set_config and source-size changes.  Host memory only: no CUDA
  * call, no device needed. */
 OVRFSR_API int ovrfsr_set_focus(ovrfsr_ctx *ctx, int eye, float x, float y);
@@ -246,6 +250,19 @@ OVRFSR_API int ovrfsr_clear_focus(ovrfsr_ctx *ctx, int eye);
 OVRFSR_API int ovrfsr_set_focus_radius(ovrfsr_ctx *ctx, int eye, float radius);
 /* back to ovrfsr_config::radius for eye; the focus stays */
 OVRFSR_API int ovrfsr_clear_focus_radius(ovrfsr_ctx *ctx, int eye);
+/* Sharpness of both eyes, in place of ovrfsr_config::sharpness, without a reset: what the sharpness hotkeys
+ * (PostProcessor.cpp:670-704) or an in-headset slider change while the game runs.  Every apply entry point gives the
+ * bytes of a ctx configured with that sharpness, in both math modes, on FSR (RCAS, alone or after EASU, fused or
+ * not, with or without OVRFSR_FLAG_SRTM) and on NIS (NVScaler, NVSharpen).  Late-latched exactly like
+ * ovrfsr_set_focus, in the same block.  Stored as given, so it survives ovrfsr_reset, ovrfsr_set_config and
+ * source-size changes; a new ovrfsr_config::sharpness takes effect after ovrfsr_clear_sharpness.  An F7 capture
+ * names its file with the override current when the capturing apply is issued.  ovrfsr_get_config,
+ * ovrfsr_get_sharpen_constants and the stateless dispatches keep reporting / using the config's sharpness.
+ * OVRFSR_ERR_INVALID for sharpness not finite or outside [0, 1]; the previous value stays.  Host memory only: any
+ * thread, concurrently with applies, before the first one too. */
+OVRFSR_API int ovrfsr_set_sharpness(ovrfsr_ctx *ctx, float sharpness);
+/* back to ovrfsr_config::sharpness */
+OVRFSR_API int ovrfsr_clear_sharpness(ovrfsr_ctx *ctx);
 
 /* ---- individual dispatches (ApplyUpscaling / ApplySharpening, PostProcessor.cpp:385-401,483-496) --
  * Stateless: explicit constant blocks, caller-owned destination.  math_mode as ovrfsr_math. */

@@ -53,6 +53,8 @@ SYMBOLS = {
     "ovrfsr_clear_focus": (C.c_int, [_vp, C.c_int]),
     "ovrfsr_set_focus_radius": (C.c_int, [_vp, C.c_int, C.c_float]),
     "ovrfsr_clear_focus_radius": (C.c_int, [_vp, C.c_int]),
+    "ovrfsr_set_sharpness": (C.c_int, [_vp, C.c_float]),
+    "ovrfsr_clear_sharpness": (C.c_int, [_vp]),
     "ovrfsr_dispatch_fsr_easu": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, _vp]),
     "ovrfsr_dispatch_fsr_rcas": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, _vp]),
     "ovrfsr_dispatch_fsr_easu_ex": (C.c_int, [_imgp, _imgp, _u32p, C.c_int, C.c_int, _vp]),

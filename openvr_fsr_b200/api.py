@@ -225,6 +225,15 @@ class PostProcessor:
         """ovrfsr_clear_focus_radius: back to Config.radius for `eye`."""
         L.check(L.lib().ovrfsr_clear_focus_radius(self._ctx, eye), "ovrfsr_clear_focus_radius", self._ctx)
 
+    def set_sharpness(self, sharpness: float):
+        """ovrfsr_set_sharpness: both eyes use `sharpness` (in [0, 1]) instead of Config.sharpness, with no reset -- the
+        bytes of a ctx configured with it.  Late-latched like set_focus; survives set_config."""
+        L.check(L.lib().ovrfsr_set_sharpness(self._ctx, sharpness), "ovrfsr_set_sharpness", self._ctx)
+
+    def clear_sharpness(self):
+        """ovrfsr_clear_sharpness: back to Config.sharpness."""
+        L.check(L.lib().ovrfsr_clear_sharpness(self._ctx), "ovrfsr_clear_sharpness", self._ctx)
+
     def apply(self, eye: int, texture, bounds: TextureBounds | None = None, fmt: int | None = None, stream=None,
               samples: int = 1):
         """vr::PostProcessor::Apply.  Returns a torch tensor VIEW of the ctx-owned output (valid until the next

@@ -14,6 +14,7 @@
 #include "array_io.h"
 #include "host_constants.h"
 #include "kernels.h"
+#include "nis_host.h"
 
 namespace ovrfsr {
 static std::atomic<uint64_t> g_launches{0};
@@ -103,23 +104,27 @@ cudaError_t expand_rgb32f(const ovrfsr_image &src, const ovrfsr_image &dst, cuda
   return cudaGetLastError();
 }
 
-// The radius mask's focus and radius (ovrfsr_set_focus, ovrfsr_set_focus_radius).  `slot` (pinned host memory, one
-// 32-byte block per eye: imageCentre[4], radiusSq[2], two words of padding) is what each apply's H2D copy reads when it
-// runs on the GPU; it is written under `mu` only, each centre pair and the radius pair with one aligned 64-bit store,
-// so a copy that overlaps an update sees whole pairs.  No CUDA call is made under `mu`.
-constexpr int kFocusWords = 8;
+// The radius mask's focus and radius and the sharpness (ovrfsr_set_focus, ovrfsr_set_focus_radius,
+// ovrfsr_set_sharpness).  `slot` (pinned host memory, one kLatchWords block per eye laid out as kernels.h describes) is
+// what each apply's H2D copy reads when it runs on the GPU; it is written under `mu` only, each pair of words with one
+// aligned 64-bit store, so a copy that overlaps an update sees whole pairs.  No CUDA call is made under `mu`.
 struct Focus {
   std::mutex mu;
   bool set[2] = {false, false};
   float xy[2][2] = {};
   bool radiusSet[2] = {false, false};
   float radius[2] = {};     // in the units of ovrfsr_config::radius
-  // what the words are computed for: the ctx's config, layout and output size at its last prepare_resources
+  bool sharpSet = false;
+  float sharpness = 0.f;    // in [0, 1]; one value for both eyes, like ovrfsr_config::sharpness
+  // what the words are computed for: the ctx's config, layout, sizes and NIS pass at its last prepare_resources
   bool ready = false;
   ovrfsr_config cfg{};
   bool onlyOneEye = true;
-  uint32_t outW = 0, outH = 0;
-  uint32_t *slot = nullptr; // [2][kFocusWords], allocated by the first apply that needs it
+  uint32_t inW = 0, inH = 0, outW = 0, outH = 0;
+  bool nisSharpenOnly = false;
+  uint32_t *slot = nullptr; // [2][kLatchWords], allocated by the first apply that needs it
+  // some eye has a focus or a radius override, or the sharpness is overridden: applies copy the slot
+  bool any() const { return set[0] || set[1] || radiusSet[0] || radiusSet[1] || sharpSet; }
 };
 
 // What every apply of a context runs (PostProcessor.cpp:586-594), decided by prepare_resources from the config, the
@@ -180,9 +185,9 @@ struct ovrfsr_ctx {
   // ovrfsr_apply_pair: the right eye's chain runs on this stream between a fork and a join event
   cudaStream_t pairStream = nullptr;
   cudaEvent_t pairFork = nullptr, pairJoin = nullptr;
-  // ovrfsr_set_focus / ovrfsr_set_focus_radius: `active` while some eye has a focus or a radius override; then each
-  // apply copies its eye's slot block into `focusDev` ([2][kFocusWords] words, device) at its head, and the masked
-  // kernels read their centre and radius words from there
+  // ovrfsr_set_focus / ovrfsr_set_focus_radius / ovrfsr_set_sharpness: `active` while some eye has a focus or a radius
+  // override or the sharpness is overridden; then each apply copies its eye's slot block into `focusDev`
+  // ([2][kLatchWords] words, device) at its head, and the kernels read their centre, radius and sharpness words from there
   Focus focus;
   std::atomic<bool> focusActive{false};
   uint32_t *focusDev = nullptr;
@@ -219,10 +224,18 @@ int select_device(ovrfsr_ctx *c) {
 // the slot's words: host::centre_radius with each focused eye's proj_centre pair replaced by its focus, and radiusSq[k]
 // the R^2 of the eye centre pair k is sourced from -- with that eye's radius override, if any, in place of cfg.radius.
 // Block e of one-eye-per-texture submits takes both words from eye e; block 0 of a shared texture takes pair 0 from the
-// left eye and pair 1 from the right (block 1 of a shared texture is never read).
+// left eye and pair 1 from the right (block 1 of a shared texture is never read).  The sharpness words of both blocks
+// are those of the config with the override, if any, in place of cfg.sharpness, made by the very functions that
+// prepare_resources builds the constant blocks with, so that they equal a configured ctx's bit for bit.
 void write_focus_slot(Focus &f) {
   if (!f.slot || !f.ready) return;
   ovrfsr_config cfg = f.cfg;
+  if (f.sharpSet) cfg.sharpness = f.sharpness;
+  uint32_t rcas[12];
+  host::make_sharpen_constants(rcas, cfg, 0, true, f.outW, f.outH);
+  host::NisConfig nis;
+  host::make_nis_config(nis, cfg, f.nisSharpenOnly, 0, true, f.inW, f.inH, f.outW, f.outH);
+  const float nisSharp[4] = {nis.kSharpStrengthMin, nis.kSharpStrengthScale, nis.kSharpLimitMin, nis.kSharpLimitScale};
   for (int e = 0; e < 2; ++e)
     if (f.set[e]) { cfg.proj_centre[2 * e] = f.xy[e][0]; cfg.proj_centre[2 * e + 1] = f.xy[e][1]; }
   uint32_t eyeRsq[2];
@@ -234,24 +247,26 @@ void write_focus_slot(Focus &f) {
     eyeRsq[e] = radius[1];
   }
   for (int b = 0; b < 2; ++b) {
-    alignas(8) uint32_t words[6];
+    alignas(8) uint32_t words[kLatchNisSharp + 4] = {};
     uint32_t radius[4];
     host::centre_radius(words, radius, cfg, b, f.onlyOneEye, f.outW, f.outH);
     words[4] = eyeRsq[f.onlyOneEye ? b : 0];
     words[5] = eyeRsq[f.onlyOneEye ? b : 1];
-    uint64_t pair[3];
+    words[kLatchRcasSharp] = rcas[0];
+    std::memcpy(words + kLatchNisSharp, nisSharp, sizeof(nisSharp));
+    uint64_t pair[(kLatchNisSharp + 4) / 2];
     std::memcpy(pair, words, sizeof(pair));
-    uint64_t *dst = reinterpret_cast<uint64_t *>(f.slot + kFocusWords * b);
-    for (int k = 0; k < 3; ++k) __atomic_store_n(&dst[k], pair[k], __ATOMIC_RELAXED);
+    uint64_t *dst = reinterpret_cast<uint64_t *>(f.slot + kLatchWords * b);
+    for (int k = 0; k < (kLatchNisSharp + 4) / 2; ++k) __atomic_store_n(&dst[k], pair[k], __ATOMIC_RELAXED);
   }
 }
 
-// head of an apply with a focus or a radius override active: copy this eye's slot block to its device block on `s`, so
-// the kernels of the apply see the words the slot holds when the copy runs (and a captured graph re-reads the slot on
-// every replay)
+// head of an apply with a focus, a radius override or a sharpness override active: copy this eye's slot block to its
+// device block on `s`, so the kernels of the apply see the words the slot holds when the copy runs (and a captured
+// graph re-reads the slot on every replay)
 int latch_focus(ovrfsr_ctx *c, int eye, cudaStream_t s, const uint32_t **centreDev) {
   Focus &f = c->focus;
-  constexpr size_t kBytes = 2 * kFocusWords * sizeof(uint32_t);
+  constexpr size_t kBytes = 2 * kLatchWords * sizeof(uint32_t);
   if (!f.slot) {
     uint32_t *slot = nullptr;
     cudaError_t e = cudaHostAlloc(reinterpret_cast<void **>(&slot), kBytes, cudaHostAllocPortable);
@@ -265,10 +280,10 @@ int latch_focus(ovrfsr_ctx *c, int eye, cudaStream_t s, const uint32_t **centreD
     cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&c->focusDev), kBytes);
     if (e != cudaSuccess) { c->focusDev = nullptr; return fail(c, OVRFSR_ERR_NOMEM, "allocating the focus block", e); }
   }
-  cudaError_t e = cudaMemcpyAsync(c->focusDev + kFocusWords * eye, f.slot + kFocusWords * eye, kFocusWords * sizeof(uint32_t),
+  cudaError_t e = cudaMemcpyAsync(c->focusDev + kLatchWords * eye, f.slot + kLatchWords * eye, kLatchWords * sizeof(uint32_t),
                                   cudaMemcpyHostToDevice, s);
   if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "focus copy", e);
-  *centreDev = c->focusDev + kFocusWords * eye;
+  *centreDev = c->focusDev + kLatchWords * eye;
   return OVRFSR_OK;
 }
 
@@ -331,10 +346,11 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
     }
     c->evCreated = true;
   }
-  { // the focus words for the new config / layout / output size (the focus itself survives resets)
+  { // the slot words for the new config / layout / sizes (the focus and the overrides themselves survive resets)
     std::lock_guard<std::mutex> lock(c->focus.mu);
     Focus &f = c->focus;
     f.cfg = c->cfg; f.onlyOneEye = one; f.outW = c->outputWidth; f.outH = c->outputHeight; f.ready = true;
+    f.inW = c->inputWidth; f.inH = c->inputHeight; f.nisSharpenOnly = !p.upscale; // the NISConfig the NIS pass takes
     write_focus_slot(f);
   }
   c->initialized = true;
@@ -354,6 +370,11 @@ void harvest_queries(ovrfsr_ctx *c) {
 
 // PostProcessor::SaveTextureToFile, PostProcessor.cpp:640-657: staging copy, then the DDS writer (capture.cpp)
 int save_capture(ovrfsr_ctx *c, const Image &img, cudaStream_t s) {
+  ovrfsr_config named = c->cfg; // the name carries the sharpness override current when the capturing apply is issued
+  {
+    std::lock_guard<std::mutex> lock(c->focus.mu);
+    if (c->focus.sharpSet) named.sharpness = c->focus.sharpness;
+  }
   const size_t rowBytes = (size_t)img.width * bytes_per_pixel(img.format);
   std::vector<uint8_t> host(rowBytes * img.height);
   cudaError_t e = img.array ? cudaMemcpy2DFromArrayAsync(host.data(), rowBytes, static_cast<cudaArray_const_t>(img.data), 0, 0, rowBytes,
@@ -362,7 +383,7 @@ int save_capture(ovrfsr_ctx *c, const Image &img, cudaStream_t s) {
   if (e == cudaSuccess) e = cudaStreamSynchronize(s);
   if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "capture read-back", e);
   char name[96];
-  if (ovrfsr_capture_filename(&c->cfg, (int64_t)std::time(nullptr), name, sizeof(name)) != OVRFSR_OK)
+  if (ovrfsr_capture_filename(&named, (int64_t)std::time(nullptr), name, sizeof(name)) != OVRFSR_OK)
     return fail(c, OVRFSR_ERR_INVALID, "capture file name");
   c->lastCapturePath = c->captureDir.empty() ? std::string(name) : c->captureDir + "/" + name;
   const ovrfsr_image h{host.data(), img.width, img.height, (uint32_t)rowBytes, img.format, 1, 0, 0};
@@ -642,7 +663,7 @@ int ovrfsr_clear_focus(ovrfsr_ctx *ctx, int eye) {
   std::lock_guard<std::mutex> lock(f.mu);
   f.set[eye] = false;
   write_focus_slot(f); // graphs captured with a focus fall back to the projection centre
-  ctx->focusActive.store(f.set[0] || f.set[1] || f.radiusSet[0] || f.radiusSet[1], std::memory_order_release);
+  ctx->focusActive.store(f.any(), std::memory_order_release);
   return OVRFSR_OK;
 }
 
@@ -664,7 +685,28 @@ int ovrfsr_clear_focus_radius(ovrfsr_ctx *ctx, int eye) {
   std::lock_guard<std::mutex> lock(f.mu);
   f.radiusSet[eye] = false;
   write_focus_slot(f); // graphs captured with an override fall back to ovrfsr_config::radius
-  ctx->focusActive.store(f.set[0] || f.set[1] || f.radiusSet[0] || f.radiusSet[1], std::memory_order_release);
+  ctx->focusActive.store(f.any(), std::memory_order_release);
+  return OVRFSR_OK;
+}
+
+int ovrfsr_set_sharpness(ovrfsr_ctx *ctx, float sharpness) {
+  if (!ctx || !(sharpness >= 0.f && sharpness <= 1.f)) return OVRFSR_ERR_INVALID;
+  Focus &f = ctx->focus;
+  std::lock_guard<std::mutex> lock(f.mu);
+  f.sharpSet = true;
+  f.sharpness = sharpness;
+  write_focus_slot(f);
+  ctx->focusActive.store(true, std::memory_order_release);
+  return OVRFSR_OK;
+}
+
+int ovrfsr_clear_sharpness(ovrfsr_ctx *ctx) {
+  if (!ctx) return OVRFSR_ERR_INVALID;
+  Focus &f = ctx->focus;
+  std::lock_guard<std::mutex> lock(f.mu);
+  f.sharpSet = false;
+  write_focus_slot(f); // graphs captured with an override fall back to ovrfsr_config::sharpness
+  ctx->focusActive.store(f.any(), std::memory_order_release);
   return OVRFSR_OK;
 }
 

@@ -37,7 +37,7 @@ struct FusedArgs {
   ImageRW dst;
   float c0x, c0y, c0z, c0w;
   uint32_t centre[4];
-  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`; else the device block holding the mask words (load_centre)
+  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`, `sharp`; else the ctx's latched block (load_centre, load_rcas_sharp)
   uint32_t radiusSq;
   float radW, radH;
   int tileW, tileH;   // shared source tile extent in texels (for the 66 x 34 region)
@@ -92,6 +92,7 @@ __global__ void __launch_bounds__(kThreads, 2) fsr_fused_kernel(const __grid_con
 
   uint32_t centre[4], rsq[2];
   load_centre(centre, rsq, a.centre, a.radiusSq, a.centreDev);
+  const float sharp = load_rcas_sharp(a.sharp, a.centreDev);
   uint32_t phase = 0;
   for (; t < numTiles; t += gridDim.x) {
     int ox0, oy0, sx0, sy0;
@@ -284,7 +285,7 @@ __global__ void __launch_bounds__(kThreads, 2) fsr_fused_kernel(const __grid_con
             for (int i = 0; i < 6; ++i) mrow[i] = mid[i - 1];
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
-              const float3 c = rcas_filter_mode<kU8>(mid[i - kFusedMS], mrow[i], mrow[i + 1], mrow[i + 2], mid[i + kFusedMS], a.sharp);
+              const float3 c = rcas_filter_mode<kU8>(mid[i - kFusedMS], mrow[i], mrow[i + 1], mrow[i + 2], mid[i + kFusedMS], sharp);
               px[i] = make_float4(c.x, c.y, c.z, 1.0f);
             }
           } else {

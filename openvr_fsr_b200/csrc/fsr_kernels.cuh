@@ -50,7 +50,7 @@ struct RcasArgs {
   float sharp;              // const0[0] as float
   float tintGB;             // 1 - debug*0.3 (fsr_rcas.hlsl:46)
   uint32_t centre[4];
-  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`; else the device block holding the mask words (load_centre)
+  const uint32_t *centreDev; // nullptr: `centre`, `radiusSq`, `sharp`; else the ctx's latched block (load_centre, load_rcas_sharp)
   uint32_t radiusSq;
   int skipOutside;          // the preceding EASU launch already wrote the outside-radius groups to dst (EasuArgs::direct)
   int opaqueSrc;            // B8G8R8X8 source: the X byte reads as alpha 1 (only the outside-radius copy looks at alpha)
@@ -754,6 +754,7 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
 
   uint32_t centre[4], rsq[2];
   load_centre(centre, rsq, a.centre, a.radiusSq, a.centreDev);
+  const float sharp = load_rcas_sharp(a.sharp, a.centreDev);
   if constexpr (PAIRED) {
     // uniform per CTA: nothing of this tile is inside the radius -> nothing to do (and no TMA load is issued)
     bool any = false;
@@ -833,7 +834,7 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       const int y = y0 + k;
       if (y >= a.dst.h) break;
       const float4 h = p[kRcasTW], d = p[-1], f = p[1];
-      float3 c = rcas_filter_mode<FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_BGRA8>(b, d, e, f, h, a.sharp);
+      float3 c = rcas_filter_mode<FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_BGRA8>(b, d, e, f, h, sharp);
       if constexpr (!packed32(FIN)) {
         if (a.srtmOut) srtm_inv(c.x, c.y, c.z); // also the value a one-colour group's other rows take
       }

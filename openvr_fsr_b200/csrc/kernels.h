@@ -12,14 +12,20 @@ namespace ovrfsr {
 // unused; `layer` selects the layer of a layered array, -1 = not layered).
 struct PassImage { void *ptr; uint32_t pitch; int w, h; int format; bool array = false; int layer = -1; };
 
+// the `centreDev` block described below: its size in words and where its sharpness words sit
+constexpr int kLatchWords = 16, kLatchRcasSharp = 6, kLatchNisSharp = 8;
+
 // FSR (fsr_kernels.cuh).  consts are the reference's constant-buffer layouts.
 // `direct` (EASU) / `skipOutside` (RCAS) are the ctx path's pairing of the two passes: when RCAS follows EASU in the same
 // apply, EASU writes the outside-radius groups -- which RCAS would only copy (x the debug tint `tintGB`) -- straight
 // to the final image `direct`, and RCAS visits only tiles / groups inside the radius.  Same output bits as two plain
 // dispatches; a stateless dispatch passes nullptr / false.
-// `centreDev` (every masked launcher): nullptr = the imageCentre and radiusSq words of the constant block; else a 32-byte
-// device block {imageCentre[4], radiusSq[2], pad[2]} the kernels read those words from when they run (the ctx path with
-// a focus or a focus radius, ovrfsr_set_focus / ovrfsr_set_focus_radius); radiusSq[k] is centre pair k's squared radius.
+// `centreDev` (every masked launcher): nullptr = the mask and sharpness words of the constant block; else a 64-byte
+// device block the kernels read those words from when they run (the ctx path with a focus, a focus radius or a
+// sharpness override: ovrfsr_set_focus / ovrfsr_set_focus_radius / ovrfsr_set_sharpness):
+//   words 0-3 imageCentre, 4-5 radiusSq of centre pair 0 / 1, 6 RCAS const0[0] (RCAS and the fused kernel),
+//   8-9 NISConfig kSharpStrengthMin / kSharpStrengthScale, 10-11 kSharpLimitMin / kSharpLimitScale (NVScaler and
+//   NVSharpen), 7 and 12-15 padding.  EASU reads words 0-5 only.
 // `srtm` (EASU and RCAS): OVRFSR_PASS_SRTM_* bits, AMD's reversible tone map on the texels read / the pixels stored.
 // Float sources only, and never together with the pairing: cudaErrorInvalidValue otherwise.
 cudaError_t launch_easu_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,

@@ -156,4 +156,15 @@ bool PostProcessor::ClearFocusRadius(EVREye eEye) {
   return c && ovrfsr_clear_focus_radius(c, eEye == Eye_Right ? 1 : 0) == OVRFSR_OK;
 }
 
+// the sharpness override lives in the ctx too: Reset and the set_config of the first Apply keep it
+bool PostProcessor::SetSharpness(float sharpness) {
+  ovrfsr_ctx *c = Context();
+  return c && ovrfsr_set_sharpness(c, sharpness) == OVRFSR_OK;
+}
+
+bool PostProcessor::ClearSharpness() {
+  ovrfsr_ctx *c = Context();
+  return c && ovrfsr_clear_sharpness(c) == OVRFSR_OK;
+}
+
 } // namespace vr

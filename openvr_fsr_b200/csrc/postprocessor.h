@@ -55,6 +55,12 @@ public:
   // SetFocus.  false: rejected (radius not finite, negative or > 4).
   bool SetFocusRadius(EVREye eEye, float radius);
   bool ClearFocusRadius(EVREye eEye);
+  // Live sharpness (ovrfsr_set_sharpness / ovrfsr_clear_sharpness): both eyes use `sharpness` instead of
+  // Config::sharpness from the next frame whose GPU work starts after the call, with no Reset -- what the sharpness
+  // hotkeys call after changing Config::sharpness.  Same threading as SetFocus.  false: rejected (not finite or
+  // outside [0, 1]).
+  bool SetSharpness(float sharpness);
+  bool ClearSharpness();
 
 private:
   ovrfsr_ctx *Context(); // creates the ctx on first use (no GPU work); guarded by ctxMutex

@@ -2,7 +2,9 @@
 (stereo 1683x1869 -> 2244x2492 RGBA8, strict FSR EASU+RCAS, the bench.py scene).  Pairs/s with the focus off, set once
 (static) and moved before every frame (moving), at radius 0.3, 0.5 and 2.0; and with a per-eye radius override equal
 to the config radius, set once with no focus (radius_static), or changed before every frame -- both eyes alternating
-0.3 / 0.5, out of phase -- with the focus moving too (radius_moving).  Two drivers:
+0.3 / 0.5, out of phase -- with the focus moving too (radius_moving); and with a sharpness override
+(ovrfsr_set_sharpness) and no focus or radius override, equal to the config sharpness and set once (sharp_static), or
+alternated 0.9 / 0.6 before every frame (sharp_moving).  Two drivers:
   pair     : one caller stream, both eyes per PostProcessor.apply_pair call
   streams4 : two contexts (frames in flight), one stream per eye -- bench.py's default driver
 Each arm is the median of --reps timed windows of --passes passes over a pool of 8 distinct pairs (CUDA events on
@@ -10,8 +12,9 @@ the caller stream, everything joined before the end event).  The focus cost per 
 between 'static' and 'off' (at radius 2.0 every group is filtered whatever the centre, so only the copy differs).
 
 A/B: --lib PATH (repeatable) runs each library in its own child process, alternated --rounds times; a library without
-ovrfsr_set_focus (an older build) runs the 'off' arms only, one without ovrfsr_set_focus_radius skips the radius_* arms.  The card's name, power limit and SM clock are read in the
-same call and printed with the numbers.
+ovrfsr_set_focus (an older build) runs the 'off' arms only, one without ovrfsr_set_focus_radius skips the radius_* arms,
+one without ovrfsr_set_sharpness the sharp_* arms.  The card's name, power limit and SM clock are read in the same
+call and printed with the numbers.
 usage: python tools/bench_foveation.py [--lib A.so --lib B.so] [--rounds 2] [--json out.json]"""
 import argparse
 import json
@@ -24,7 +27,7 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parents[1]
 IN_W, IN_H, SCALE, SHARP, POOL = 1683, 1869, 0.75, 0.9, 8
 RADII = (0.3, 0.5, 2.0)
-FOCUS = ("off", "static", "moving", "radius_static", "radius_moving")
+FOCUS = ("off", "static", "moving", "radius_static", "radius_moving", "sharp_static", "sharp_moving")
 DRIVERS = ("pair", "streams4")
 
 
@@ -42,6 +45,7 @@ def child(args):
     dev = torch.device("cuda:0")
     has_focus = hasattr(L.lib(), "ovrfsr_set_focus")
     has_radius = hasattr(L.lib(), "ovrfsr_set_focus_radius")
+    has_sharp = hasattr(L.lib(), "ovrfsr_set_sharpness")
     base_l, base_r = synth.stereo_pair("natural", IN_W, IN_H, 1)
     pool = [(ovr.to_image(np.roll(base_l, 37 * i, axis=0), dev), ovr.to_image(np.roll(base_r, 37 * i, axis=0), dev))
             for i in range(POOL)]
@@ -54,11 +58,15 @@ def child(args):
             pps = [ovr.PostProcessor(cfg) for _ in range(n_ctx)]
             streams = [[main, main]] if driver == "pair" else [[torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)] for _ in pps]
             for focus in FOCUS:
-                if (focus != "off" and not has_focus) or (focus.startswith("radius") and not has_radius):
+                if ((focus != "off" and not has_focus) or (focus.startswith("radius") and not has_radius) or
+                        (focus.startswith("sharp") and not has_sharp)):
                     continue
                 for p in pps:
-                    if focus in ("off", "radius_static") and has_focus:
+                    if focus in ("off", "radius_static", "sharp_static", "sharp_moving") and has_focus:
                         p.clear_focus(0), p.clear_focus(1)
+                    if focus.startswith("sharp"):
+                        p.clear_focus_radius(0), p.clear_focus_radius(1)
+                        p.set_sharpness(SHARP)
                     if focus == "static":
                         p.set_focus(0, 0.45, 0.55), p.set_focus(1, 0.55, 0.55)
                     elif focus == "radius_static":
@@ -73,6 +81,8 @@ def child(args):
                             p.set_focus(0, *gaze(i)), p.set_focus(1, *gaze(i + 1))
                         if focus == "radius_moving":
                             p.set_focus_radius(0, (0.3, 0.5)[i % 2]), p.set_focus_radius(1, (0.5, 0.3)[i % 2])
+                        if focus == "sharp_moving":
+                            p.set_sharpness((SHARP, 0.6)[i % 2])
                         if driver == "pair":
                             p.apply_pair(l, r, stream=sl)
                         else:
@@ -94,7 +104,7 @@ def child(args):
             for p in pps:
                 p.close()
     print(json.dumps({"lib": os.environ.get("OVRFSR_LIB", "in-tree"), "has_focus": has_focus, "has_radius": has_radius,
-                      "arms": res}))
+                      "has_sharp": has_sharp, "arms": res}))
 
 
 def card():

@@ -2,7 +2,9 @@
 2016x2240, sharpness 0.9, NVScaler only) and of NVSharpen at 2016x2240.  CUDA events on the launch stream, no sync
 inside the loop.  Both kernels skip the directional filters of pixels whose interpolated edge weights are all zero, so
 their time depends on the CONTENT: measured on the natural scene (1-2 % of the texels carry an edge), the textured one
-(about a third) and uniform noise (84 %: nothing to skip).  usage: python tools/bench_nis.py [--math fast|strict]"""
+(about a third) and uniform noise (84 %: nothing to skip).  The *_ctx arms time the kernels of the ctx path, with and
+without the latched block of ovrfsr_set_sharpness (torch.profiler, per launch).
+usage: python tools/bench_nis.py [--math fast|strict]"""
 import argparse, json, statistics, sys
 from pathlib import Path
 import numpy as np, torch
@@ -38,4 +40,30 @@ for content, radius in (("natural", 2.0), ("natural", 0.5), ("textured", 2.0), (
         torch.cuda.synchronize()
         ms = statistics.mean(x.elapsed_time(y) for x, y in marks[len(marks) // 4:])
         out[f"{name}_r{radius}{sfx}"] = {"ms_per_eye": ms, "GBps_algorithmic": nbytes / ms / 1e6, "eye_pairs_per_s_1gpu": 500.0 / ms}
+
+# The ctx path with and without the latched block (a sharpness override equal to the config's makes the kernels read
+# their mask and sharpness words from the block the apply's 64-byte copy refreshes): kernel time per launch from
+# torch.profiler, so the copy itself is not counted.  Natural scene, radius 2.0 and 0.5.
+def ctx_kernel_us(cfg, srcs, latched):
+    pp = ovr.PostProcessor(cfg)
+    if latched:
+        pp.set_sharpness(cfg.sharpness)
+    for s in srcs: pp.apply(0, s)
+    torch.cuda.synchronize()
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for _ in range(a.reps):
+            for s in srcs: pp.apply(0, s)
+        torch.cuda.synchronize()
+    pp.close()
+    times = [e.time_range.elapsed_us() for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "nis_" in e.name]
+    return statistics.median(times), len(times)
+
+
+for radius in (2.0, 0.5):
+    for name, sc, srcs in (("nvscaler", scale, [ovr.to_image(np.roll(synth.natural_rgba8(iw, ih, 1), 31 * i, axis=0), dev) for i in range(8)]),
+                           ("nvsharpen", 1.0, [ovr.to_image(np.roll(synth.natural_rgba8(ow, oh, 2), 31 * i, axis=0), dev) for i in range(4)])):
+        cfg = ovr.Config(fsrEnabled=True, useNis=True, renderScale=sc, sharpness=0.9, radius=radius, mathMode=mode)
+        for latched in (False, True):
+            us, n = ctx_kernel_us(cfg, srcs, latched)
+            out[f"{name}_ctx{'_latched' if latched else ''}_r{radius}"] = {"us_per_launch_median": us, "launches": n}
 print(json.dumps({"workload": "C4 1512x1680->2016x2240 RGBA8 NIS sharpness 0.9", "math": a.math, **out}))
