@@ -402,22 +402,31 @@ __device__ __forceinline__ int easu_flat_group(const float4 *__restrict__ sC, co
 constexpr int kEasuRowsPerThread = 5;  // tile rows handled by one warp: ceil(37 / 8)
 constexpr int kEasuColsPerThread = 3;  // 32-wide column blocks: ceil(72 / 32)
 
+// Resident CTAs per SM that ptxas budgets registers for (64 per thread at 4, 80 at 3).  The tile takes 32 B per texel
+// (60 x 29 x 32 = 55,680 B at C2), so four fit at the 60-texel stride, and strict math needs 62 registers there.  Fast
+// math needs ~78 and stays at three; so does the 72-texel stride, whose tile does not fit four times.
+constexpr int easu_min_ctas(int tw) { return kStrict && tw == 60 ? 4 : 3; }
+
 // PAIRED = RCAS follows in the same apply (EasuArgs::direct is set): a compile-time variant, so that the plain dispatch
 // keeps exactly the instruction stream it had without the pairing.
 // ANYIO = any of src (TMA == false only), dst and direct may be a CUDA array (`io`); otherwise `io` is unused.
 template <int FIN, int FOUT, int TW, bool TMA, bool PAIRED, bool ANYIO>
-__global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant__ EasuArgs a,
-                                                           const __grid_constant__ CUtensorMap srcMap,
-                                                           const __grid_constant__ ArrayIO io) {
-  extern __shared__ __align__(128) uint8_t smem_raw[];
+__global__ void __launch_bounds__(kThreads, easu_min_ctas(TW)) easu_kernel(const __grid_constant__ EasuArgs a,
+                                                                           const __grid_constant__ CUtensorMap srcMap,
+                                                                           const __grid_constant__ ArrayIO io) {
+  extern __shared__ __align__(128) uint8_t smem_raw[]; // 32 B per tile texel (easu_launch_t)
   __shared__ uint64_t tileBar;
   __shared__ BilinAxis sRowAxis[kTileH]; // Bilinear()'s row terms of this tile (outside-radius groups only)
   const int th = a.tileH, tn = TW * th;
   float4 *sC = reinterpret_cast<float4 *>(smem_raw);  // decoded colour (r,g,b,1)
   float4 *sF = sC + tn;                               // (dirX, dirY, lenX, lenY) per texel
-  float *sL = reinterpret_cast<float *>(sF + tn);     // luma*2 plane (conflict-free stencil reads)
+  // The luma*2 plane (conflict-free stencil reads) and the TMA landing zone live in the feature tile until stage 2
+  // writes it: the landing zone is read by stage 1 only, and stage 2 holds every luma it needs in registers before it
+  // writes a feature.  The landing zone is 128-byte aligned (a misaligned bulk-tensor destination faults) and, as
+  // rawW <= TW, ends inside sF.
+  float *sL = reinterpret_cast<float *>(sF);
   const int rawW = a.tileW + 4;                       // TMA box width (origin floored to 4 texels)
-  uint32_t *sRaw = reinterpret_cast<uint32_t *>(smem_raw + ((tn * 36 + 127) & ~127)); // landing zone (TMA only), 128-byte aligned
+  uint32_t *sRaw = reinterpret_cast<uint32_t *>(smem_raw + ((tn * 20 + 127) & ~127));
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 
@@ -514,24 +523,34 @@ __global__ void __launch_bounds__(kThreads, 3) easu_kernel(const __grid_constant
 
   // ---- stage 2: per-source-texel direction/length features (only where EASU will run) -----------
   if (anyFilter) {
+    // Each warp walks a run of consecutive rows, so a lane loads its column's lumas once: 3 + 2 / run loads per texel.
+    constexpr int kCols = (TW + 31) / 32; // 32-wide column blocks that reach tx = cols - 2 <= TW - 2
+    const int run = (th - 2 + 7) >> 3;    // <= kEasuRowsPerThread
+    const int y0 = 1 + warp * run, n = min(run, th - 1 - y0);
+    float lV[kCols][kEasuRowsPerThread + 2], lB[kCols][kEasuRowsPerThread], lD[kCols][kEasuRowsPerThread];
 #pragma unroll
-    for (int i = 0; i < kEasuColsPerThread; ++i) {
+    for (int i = 0; i < kCols; ++i) {
       const int tx = 1 + lane + 32 * i;
-      if (tx < cols - 1) {
-        float lA[kEasuRowsPerThread], lB[kEasuRowsPerThread], lC[kEasuRowsPerThread], lD[kEasuRowsPerThread],
-            lE[kEasuRowsPerThread];
+      if (tx < cols - 1 && n > 0) {
+        const float *l = sL + y0 * TW + tx;
 #pragma unroll
-        for (int j = 0; j < kEasuRowsPerThread; ++j) {
-          const int ty = 1 + warp + 8 * j;
-          if (ty < th - 1) {
-            const float *l = sL + ty * TW + tx;
-            lA[j] = l[-TW]; lB[j] = l[-1]; lC[j] = l[0]; lD[j] = l[1]; lE[j] = l[TW];
-          }
+        for (int j = 0; j < kEasuRowsPerThread + 2; ++j) {
+          if (j <= n + 1) lV[i][j] = l[(j - 1) * TW];
         }
 #pragma unroll
         for (int j = 0; j < kEasuRowsPerThread; ++j) {
-          const int ty = 1 + warp + 8 * j;
-          if (ty < th - 1) sF[ty * TW + tx] = easu_feature(lA[j], lB[j], lC[j], lD[j], lE[j]);
+          if (j < n) { lB[i][j] = l[j * TW - 1]; lD[i][j] = l[j * TW + 1]; }
+        }
+      }
+    }
+    __syncthreads(); // the features overwrite the luma plane
+#pragma unroll
+    for (int i = 0; i < kCols; ++i) {
+      const int tx = 1 + lane + 32 * i;
+      if (tx < cols - 1 && n > 0) {
+#pragma unroll
+        for (int j = 0; j < kEasuRowsPerThread; ++j) {
+          if (j < n) sF[(y0 + j) * TW + tx] = easu_feature(lV[i][j], lB[i][j], lV[i][j + 1], lD[i][j], lV[i][j + 2]);
         }
       }
     }
