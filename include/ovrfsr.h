@@ -155,6 +155,19 @@ typedef struct ovrfsr_config {
  * whatever IEEE arithmetic gives (e.g. max3 = -1 divides by zero).  Changing the bit through ovrfsr_set_config resets
  * the ctx like any config change. */
 #define OVRFSR_FLAG_SRTM 2
+/* The same tone map around the NIS pass (NVScaler or NVSharpen), an extension the reference never enables.
+ * NVScalerUpdateConfig tunes the edge threshold kDetectThres, the contrast ratios and the sharpening strengths and
+ * limits kSharpStrength* / kSharpLimit* for luma in [0, 1]; the passes then add a luma correction to the bilinear
+ * colour, and above 1 the limiter no longer limits, so linear HDR highlights ring.  With this bit, on the NIS path with a
+ * float source (RGBA16F, RGBA32F, RGB32F after its expansion, a multisampled one after its resolve), F is applied to
+ * every source texel right after its decode and G to every stored pixel right before its encode: the pass filters
+ * F(source), and outside the radius the copy is G(tint x bilinear(F(texels))), close to a copy but not bit-exact.  Same
+ * maps, same arithmetic and same out-of-domain behaviour as OVRFSR_FLAG_SRTM; alpha untouched.  A NIS pass is a single
+ * pass, so there is no intermediate: the output keeps the ctx's output format.  Ignored -- same output bits as with the
+ * bit clear -- for UNORM sources and on the FSR path.  OVRFSR_FLAG_SRTM keeps its meaning and is still ignored on NIS;
+ * a config with both bits tone-maps whichever path runs (a host with a use_nis toggle).  This is not the NIS SDK's
+ * NIS_HDR_MODE_LINEAR / _PQ.  Changing the bit through ovrfsr_set_config resets the ctx like any config change. */
+#define OVRFSR_FLAG_SRTM_NIS 4
 
 typedef struct ovrfsr_ctx ovrfsr_ctx;
 
@@ -296,6 +309,14 @@ OVRFSR_API int ovrfsr_dispatch_nis_scaler(const ovrfsr_image *src, const ovrfsr_
                                           int math_mode, void *stream);
 OVRFSR_API int ovrfsr_dispatch_nis_sharpen(const ovrfsr_image *src, const ovrfsr_image *dst, const void *cfg256,
                                            int math_mode, void *stream);
+/* The two NIS dispatches above with the tone map of OVRFSR_FLAG_SRTM_NIS (pass_flags, OR of OVRFSR_PASS_SRTM_IN / _OUT):
+ * F after the decode of every texel the pass reads, G before the encode of every pixel it stores.  The ctx runs its one
+ * NIS pass with both bits.  pass_flags == 0 launches exactly what ovrfsr_dispatch_nis_scaler / _sharpen launch.
+ * OVRFSR_ERR_UNSUPPORTED for either bit with a UNORM source, OVRFSR_ERR_INVALID for unknown bits. */
+OVRFSR_API int ovrfsr_dispatch_nis_scaler_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const void *cfg256,
+                                             int math_mode, int pass_flags, void *stream);
+OVRFSR_API int ovrfsr_dispatch_nis_sharpen_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const void *cfg256,
+                                              int math_mode, int pass_flags, void *stream);
 
 /* ---- host-side constant setup (pure CPU; usable without a GPU) -------------------------- */
 /* PrepareResources, PostProcessor.cpp:509-518 */

@@ -19,7 +19,8 @@ FORMAT_ARRAY_BIT = 0x400  # data is a cudaArray_t
 MATH_FAST, MATH_STRICT = 0, 1
 FLAG_FUSED_FSR = 1
 FLAG_SRTM = 2  # AMD's reversible tone map around the FSR passes of a float source
-PASS_SRTM_IN, PASS_SRTM_OUT = 1, 2  # pass_flags of ovrfsr_dispatch_fsr_easu_ex / _rcas_ex
+FLAG_SRTM_NIS = 4  # the same tone map around the NIS pass of a float source
+PASS_SRTM_IN, PASS_SRTM_OUT = 1, 2  # pass_flags of ovrfsr_dispatch_{fsr_easu,fsr_rcas,nis_scaler,nis_sharpen}_ex
 
 
 class Image(C.Structure):
@@ -62,6 +63,8 @@ SYMBOLS = {
     "ovrfsr_dispatch_fsr_fused": (C.c_int, [_imgp, _imgp, _u32p, _u32p, C.c_int, _vp]),
     "ovrfsr_dispatch_nis_scaler": (C.c_int, [_imgp, _imgp, _vp, C.c_int, _vp]),
     "ovrfsr_dispatch_nis_sharpen": (C.c_int, [_imgp, _imgp, _vp, C.c_int, _vp]),
+    "ovrfsr_dispatch_nis_scaler_ex": (C.c_int, [_imgp, _imgp, _vp, C.c_int, C.c_int, _vp]),
+    "ovrfsr_dispatch_nis_sharpen_ex": (C.c_int, [_imgp, _imgp, _vp, C.c_int, C.c_int, _vp]),
     "ovrfsr_output_size": (None, [C.c_uint32, C.c_uint32, C.c_float, _u32p, _u32p]),
     "ovrfsr_fsr_easu_con": (None, [_u32p] + [C.c_float] * 6),
     "ovrfsr_fsr_rcas_con": (None, [_u32p, C.c_float]),

@@ -30,6 +30,7 @@ class Config:
     mathMode: int = L.MATH_STRICT
     fusedFsr: bool = False  # OVRFSR_FLAG_FUSED_FSR: one fused EASU->RCAS kernel instead of the two dispatches
     srtm: bool = False      # OVRFSR_FLAG_SRTM: FSR on a float (HDR) source runs between AMD's reversible tone map and its inverse
+    srtmNis: bool = False   # OVRFSR_FLAG_SRTM_NIS: NIS on a float (HDR) source runs between the same tone map and its inverse
 
     def to_c(self) -> L.Config:
         c = L.Config()
@@ -39,7 +40,8 @@ class Config:
         c.debug_mode = int(self.debugMode)
         c.proj_centre = (C.c_float * 4)(*self.projCentre)
         c.device, c.output_format, c.math_mode = self.device, self.outputFormat, self.mathMode
-        c.flags = (L.FLAG_FUSED_FSR if self.fusedFsr else 0) | (L.FLAG_SRTM if self.srtm else 0)
+        c.flags = (L.FLAG_FUSED_FSR if self.fusedFsr else 0) | (L.FLAG_SRTM if self.srtm else 0) | \
+            (L.FLAG_SRTM_NIS if self.srtmNis else 0)
         return c
 
 
@@ -389,13 +391,22 @@ def fsr_fused(src, dst, consts24, consts12, math_mode=L.MATH_STRICT, stream=None
     return dst
 
 
-def nis_scaler(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None):
+def nis_scaler(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False):
+    """g_NISUpscaleShader.  srtm_in / srtm_out (float sources only): AMD's reversible tone map on every texel read / its
+    inverse on every pixel stored (ovrfsr_dispatch_nis_scaler_ex)"""
     buf = C.create_string_buffer(bytes(cfg256), 256)
+    if srtm_in or srtm_out:
+        return _dispatch_ex(L.lib().ovrfsr_dispatch_nis_scaler_ex, src, dst, C.cast(buf, C.c_void_p), math_mode,
+                            _pass_flags(srtm_in, srtm_out), stream, src_fmt, dst_fmt)
     return _dispatch(L.lib().ovrfsr_dispatch_nis_scaler, src, dst, C.cast(buf, C.c_void_p), math_mode, stream, src_fmt, dst_fmt)
 
 
-def nis_sharpen(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None):
+def nis_sharpen(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False):
+    """g_NISSharpenShader.  srtm_in / srtm_out as for nis_scaler (ovrfsr_dispatch_nis_sharpen_ex)"""
     buf = C.create_string_buffer(bytes(cfg256), 256)
+    if srtm_in or srtm_out:
+        return _dispatch_ex(L.lib().ovrfsr_dispatch_nis_sharpen_ex, src, dst, C.cast(buf, C.c_void_p), math_mode,
+                            _pass_flags(srtm_in, srtm_out), stream, src_fmt, dst_fmt)
     return _dispatch(L.lib().ovrfsr_dispatch_nis_sharpen, src, dst, C.cast(buf, C.c_void_p), math_mode, stream, src_fmt, dst_fmt)
 
 

@@ -142,6 +142,7 @@ struct Plan {
   bool paired = false;
   bool tryFused = false;          // paired and OVRFSR_FLAG_FUSED_FSR: one fused kernel, where the images allow it
   int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* of each FSR pass
+  int nisSrtm = 0;                // OVRFSR_PASS_SRTM_* of the NIS pass
   int midFormat = OVRFSR_FORMAT_RGBA8; // of FSR's upscaled image
 };
 
@@ -307,9 +308,12 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
   p.upscale = c->cfg.render_scale != 1.f;
   const bool unormOut = c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2;
   // OVRFSR_FLAG_SRTM takes effect on the FSR path with a float source (an RGB32F one is read through its RGBA32F copy, a
-  // multisampled one after its resolve); UNORM sources are display-referred already and NIS has HDR modes of its own
-  const bool srtm = !p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM) &&
-                    (src->format == OVRFSR_FORMAT_RGBA16F || src->format == OVRFSR_FORMAT_RGBA32F || src->format == OVRFSR_FORMAT_RGB32F);
+  // multisampled one after its resolve), OVRFSR_FLAG_SRTM_NIS on the NIS path with one; UNORM sources are
+  // display-referred already
+  const bool floatSrc = src->format == OVRFSR_FORMAT_RGBA16F || src->format == OVRFSR_FORMAT_RGBA32F || src->format == OVRFSR_FORMAT_RGB32F;
+  const bool srtm = !p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM) && floatSrc;
+  // NIS runs one pass: F on every texel it reads, G on every pixel it stores
+  p.nisSrtm = p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM_NIS) && floatSrc ? OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT : 0;
   p.paired = !p.nis && p.upscale && unormOut && !srtm;
   p.tryFused = p.paired && (c->cfg.flags & OVRFSR_FLAG_FUSED_FSR);
   // SRTM: EASU applies F on read and stores tone-mapped values, RCAS applies G on store, and F on read too when it is
@@ -447,7 +451,8 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
     else if (e != cudaErrorInvalidValue && e != cudaErrorInvalidConfiguration) return fail(c, OVRFSR_ERR_CUDA, "fused EASU+RCAS launch", e);
   }
   if (p.nis) {
-    e = launch_nis(!p.upscale, in, finPass, p.upscale ? c->nisScalerConfig[eye] : c->nisSharpenConfig[eye], c->cfg.math_mode, s, centreDev);
+    e = launch_nis(!p.upscale, in, finPass, p.upscale ? c->nisScalerConfig[eye] : c->nisSharpenConfig[eye], c->cfg.math_mode, s, centreDev,
+                   p.nisSrtm);
     if (e != cudaSuccess)
       return fail(c, (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA,
                   p.upscale ? "NIS scaler dispatch" : "NIS sharpen dispatch", e);

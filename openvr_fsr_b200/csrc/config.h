@@ -19,6 +19,7 @@ struct Config {
   bool strictMath = true;   // bit-identical to the reference lines (the library default); false = FMA-contracted kernels, <= 1 LSB per pass
   bool fusedFsr = false;    // OVRFSR_FLAG_FUSED_FSR: one fused EASU->RCAS kernel instead of the two dispatches
   bool srtm = false;        // OVRFSR_FLAG_SRTM: FSR on a float (HDR) eye texture runs inside AMD's reversible tone map
+  bool srtmNis = false;     // OVRFSR_FLAG_SRTM_NIS: NIS on a float (HDR) eye texture runs inside the same tone map
 
   // ONE instance per process, owned by libovrfsr.so (an inline function-local static would be duplicated in every
   // module that includes this header when the library is built with hidden visibility)

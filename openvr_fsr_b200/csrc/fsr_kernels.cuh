@@ -57,21 +57,6 @@ struct RcasArgs {
   int srtmIn, srtmOut;      // float sources only: srtm_fwd on every texel read / srtm_inv on every pixel stored
 };
 
-// AMD's simple reversible tone mapper (ffx_fsr1.h, FsrSrtmF / FsrSrtmInvF), the opt-in HDR extension of both passes:
-// F(c) = c / (max3(c.rgb) + 1) maps linear [0, FP16_MAX] into [0, 1), where EASU's luma analysis and RCAS's limiter
-// are valid; G(c) = c / max(1/32768, 1 - max3(c.rgb)) maps back (peak 32768).  Alpha is untouched.  IEEE reciprocal in
-// both math modes: G amplifies any error near 1.  Texels outside F's domain (negative, NaN, +-inf, max3 <= -1) go
-// through the same formula; what IEEE arithmetic gives is the result.  max3 uses fmaxf, the pinned min / max rule, so
-// the operand order does not matter.  Only float-source instantiations ever contain these (if constexpr on FIN).
-__device__ __forceinline__ void srtm_fwd(float &r, float &g, float &b) {
-  const float k = __frcp_rn(__fadd_rn(fmaxf(fmaxf(r, g), b), 1.0f));
-  r = __fmul_rn(r, k); g = __fmul_rn(g, k); b = __fmul_rn(b, k);
-}
-__device__ __forceinline__ void srtm_inv(float &r, float &g, float &b) {
-  const float k = __frcp_rn(fmaxf((float)(1.0 / 32768.0), __fsub_rn(1.0f, fmaxf(fmaxf(r, g), b))));
-  r = __fmul_rn(r, k); g = __fmul_rn(g, k); b = __fmul_rn(b, k);
-}
-
 // out pixel -> source position; the same instruction sequence is used for the tile origin and
 // for every pixel so that both agree to the bit.
 __device__ __forceinline__ float easu_pos(int p, float scale, float offs) { return mul_add_unfused((float)p, scale, offs); }

@@ -48,17 +48,19 @@ cudaError_t launch_fsr_fused_strict(const PassImage &src, const PassImage &dst, 
                                     const uint32_t *centreDev = nullptr);
 
 // NIS (nis_kernels.cuh).  cfg = the 256-byte NISConfig block; coef = [2][64][8] floats (scale, usm) on the host.
+// `srtm`: OVRFSR_PASS_SRTM_* bits as for EASU and RCAS (OVRFSR_FLAG_SRTM_NIS).  Float sources only: cudaErrorInvalidValue
+// otherwise.
 cudaError_t launch_nis_scaler_fast(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
-                                   const uint32_t *centreDev = nullptr);
+                                   const uint32_t *centreDev = nullptr, int srtm = 0);
 cudaError_t launch_nis_scaler_strict(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
-                                     const uint32_t *centreDev = nullptr);
+                                     const uint32_t *centreDev = nullptr, int srtm = 0);
 cudaError_t launch_nis_sharpen_fast(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
-                                    const uint32_t *centreDev = nullptr);
+                                    const uint32_t *centreDev = nullptr, int srtm = 0);
 cudaError_t launch_nis_sharpen_strict(const PassImage &src, const PassImage &dst, const void *cfg256, const float *coef, cudaStream_t s,
-                                      const uint32_t *centreDev = nullptr);
+                                      const uint32_t *centreDev = nullptr, int srtm = 0);
 // NVScaler (sharpenOnly false) or NVSharpen with this library's filter banks, on images already validated (nis_capi.cu)
 cudaError_t launch_nis(bool sharpenOnly, const PassImage &src, const PassImage &dst, const void *cfg256, int mathMode, cudaStream_t s,
-                       const uint32_t *centreDev = nullptr);
+                       const uint32_t *centreDev = nullptr, int srtm = 0);
 
 // legacy CAS (cas_kernels.cuh).  consts = const0, const1 of src/cas/cas.compute.h:1-4 as CasSetup fills them.
 cudaError_t launch_cas_fast(const PassImage &src, const PassImage &dst, const uint32_t consts[8], int sharpenOnly, cudaStream_t s);

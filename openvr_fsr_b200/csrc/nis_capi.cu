@@ -49,6 +49,12 @@ int check(const Image *im, bool isDst) {
       reinterpret_cast<uintptr_t>(im->data) % bpp(im->format)) return OVRFSR_ERR_INVALID;
   return OVRFSR_OK;
 }
+// OVRFSR_PASS_SRTM_* of a stateless NIS dispatch, on an image check() accepted: the tone map needs a float source
+int check_pass_flags(const Image &src, int pass_flags) {
+  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT)) return OVRFSR_ERR_INVALID;
+  if (pass_flags && src.format != OVRFSR_FORMAT_RGBA16F && src.format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
+  return OVRFSR_OK;
+}
 int status_of(cudaError_t e) {
   if (e == cudaSuccess) return OVRFSR_OK;
   return (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA;
@@ -56,41 +62,56 @@ int status_of(cudaError_t e) {
 } // namespace
 
 cudaError_t ovrfsr::launch_nis(bool sharpenOnly, const PassImage &src, const PassImage &dst, const void *cfg256, int mathMode,
-                               cudaStream_t s, const uint32_t *centreDev) {
+                               cudaStream_t s, const uint32_t *centreDev, int srtm) {
   const bool strict = mathMode == OVRFSR_MATH_STRICT;
   if (sharpenOnly)
-    return strict ? launch_nis_sharpen_strict(src, dst, cfg256, nullptr, s, centreDev) : launch_nis_sharpen_fast(src, dst, cfg256, nullptr, s, centreDev);
+    return strict ? launch_nis_sharpen_strict(src, dst, cfg256, nullptr, s, centreDev, srtm)
+                  : launch_nis_sharpen_fast(src, dst, cfg256, nullptr, s, centreDev, srtm);
   const float *coef = ovrfsr_nis_coef_scale(); // g_coefScale and g_coefUsm are contiguous? no: upload buffer below
   static float both[2][64 * 8];
   static std::once_flag once;
   std::call_once(once, [&] { std::memcpy(both[0], coef, sizeof(both[0])); std::memcpy(both[1], ovrfsr_nis_coef_usm(), sizeof(both[1])); });
-  return strict ? launch_nis_scaler_strict(src, dst, cfg256, &both[0][0], s, centreDev)
-                : launch_nis_scaler_fast(src, dst, cfg256, &both[0][0], s, centreDev);
+  return strict ? launch_nis_scaler_strict(src, dst, cfg256, &both[0][0], s, centreDev, srtm)
+                : launch_nis_scaler_fast(src, dst, cfg256, &both[0][0], s, centreDev, srtm);
 }
 
 extern "C" {
 
 int ovrfsr_dispatch_nis_scaler(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
                                void *stream) {
-  Image src_u{}, dst_u{};
-  if (src_tagged) src_u = untagged(*src_tagged);
-  if (dst_tagged) dst_u = untagged(*dst_tagged, false);
-  if (!cfg256) return OVRFSR_ERR_INVALID;
-  int rc = check(src_tagged ? &src_u : nullptr, false);
-  if (rc != OVRFSR_OK || (rc = check(dst_tagged ? &dst_u : nullptr, true)) != OVRFSR_OK) return rc;
-  return status_of(launch_nis(false, pass_image(src_u), pass_image(dst_u), cfg256, math_mode, static_cast<cudaStream_t>(stream)));
+  return ovrfsr_dispatch_nis_scaler_ex(src_tagged, dst_tagged, cfg256, math_mode, 0, stream);
 }
 
 int ovrfsr_dispatch_nis_sharpen(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
                                 void *stream) {
+  return ovrfsr_dispatch_nis_sharpen_ex(src_tagged, dst_tagged, cfg256, math_mode, 0, stream);
+}
+
+int ovrfsr_dispatch_nis_scaler_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                                  int pass_flags, void *stream) {
   Image src_u{}, dst_u{};
   if (src_tagged) src_u = untagged(*src_tagged);
   if (dst_tagged) dst_u = untagged(*dst_tagged, false);
   if (!cfg256) return OVRFSR_ERR_INVALID;
   int rc = check(src_tagged ? &src_u : nullptr, false);
   if (rc != OVRFSR_OK || (rc = check(dst_tagged ? &dst_u : nullptr, true)) != OVRFSR_OK) return rc;
+  if ((rc = check_pass_flags(src_u, pass_flags)) != OVRFSR_OK) return rc;
+  return status_of(launch_nis(false, pass_image(src_u), pass_image(dst_u), cfg256, math_mode, static_cast<cudaStream_t>(stream),
+                              nullptr, pass_flags));
+}
+
+int ovrfsr_dispatch_nis_sharpen_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                                   int pass_flags, void *stream) {
+  Image src_u{}, dst_u{};
+  if (src_tagged) src_u = untagged(*src_tagged);
+  if (dst_tagged) dst_u = untagged(*dst_tagged, false);
+  if (!cfg256) return OVRFSR_ERR_INVALID;
+  int rc = check(src_tagged ? &src_u : nullptr, false);
+  if (rc != OVRFSR_OK || (rc = check(dst_tagged ? &dst_u : nullptr, true)) != OVRFSR_OK) return rc;
+  if ((rc = check_pass_flags(src_u, pass_flags)) != OVRFSR_OK) return rc;
   if (src_u.width != dst_u.width || src_u.height != dst_u.height) return OVRFSR_ERR_INVALID;
-  return status_of(launch_nis(true, pass_image(src_u), pass_image(dst_u), cfg256, math_mode, static_cast<cudaStream_t>(stream)));
+  return status_of(launch_nis(true, pass_image(src_u), pass_image(dst_u), cfg256, math_mode, static_cast<cudaStream_t>(stream),
+                              nullptr, pass_flags));
 }
 
 } // extern "C"
