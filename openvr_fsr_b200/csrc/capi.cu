@@ -440,19 +440,18 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
   const Plan &p = c->plan;
   const Image &fin = dst ? *dst : c->output[eye].img;
   const PassImage finPass = pass_image(fin);
-  const bool strict = c->cfg.math_mode == OVRFSR_MATH_STRICT;
+  const Launchers &L = launchers(c->cfg.math_mode);
   bool fused = false;
   // the fused kernel has no array I/O: with an array source or destination the two dispatches run
   if (p.tryFused && !src->array && !fin.array) {
     // EASU and RCAS as one kernel; shapes it does not cover take the two dispatches below
-    e = strict ? launch_fsr_fused_strict(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev)
-               : launch_fsr_fused_fast(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev);
+    e = L.fsr_fused(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev);
     if (e == cudaSuccess) fused = true;
     else if (e != cudaErrorInvalidValue && e != cudaErrorInvalidConfiguration) return fail(c, OVRFSR_ERR_CUDA, "fused EASU+RCAS launch", e);
   }
   if (p.nis) {
-    e = launch_nis(!p.upscale, in, finPass, p.upscale ? c->nisScalerConfig[eye] : c->nisSharpenConfig[eye], c->cfg.math_mode, s, centreDev,
-                   p.nisSrtm);
+    e = (p.upscale ? L.nis_scaler : L.nis_sharpen)(in, finPass, p.upscale ? c->nisScalerConfig[eye] : c->nisSharpenConfig[eye], s,
+                                                    centreDev, p.nisSrtm);
     if (e != cudaSuccess)
       return fail(c, (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA,
                   p.upscale ? "NIS scaler dispatch" : "NIS sharpen dispatch", e);
@@ -463,13 +462,11 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
         return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
       const PassImage *direct = p.paired ? &finPass : nullptr;
       const float tint = 1.0f - (float)c->sharpenConstants[eye][3] * 0.3f;
-      e = strict ? launch_easu_strict(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuSrtm)
-                 : launch_easu_fast(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuSrtm);
+      e = L.easu(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuSrtm);
       if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "EASU launch", e);
       in = pass_image(up.img);
     }
-    e = strict ? launch_rcas_strict(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasSrtm)
-               : launch_rcas_fast(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasSrtm);
+    e = L.rcas(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasSrtm);
     if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "RCAS launch", e);
   }
   if (q >= 0) { cudaEventRecord(c->evEnd[q], s); c->evPending[q] = true; }
@@ -834,7 +831,7 @@ int ovrfsr_format_considered_srgb(int32_t f) {
   return 0;
 }
 
-// ---- stateless dispatches ---------------------------------------------------------------------
+// ---- stateless dispatches (ApplyUpscaling / ApplySharpening, PostProcessor.cpp:385-401,483-496) --------------
 static int check_pair(const Image *src, const Image *dst) {
   int rc = validate_image(src);
   if (rc != OVRFSR_OK) return rc;
@@ -847,6 +844,33 @@ static int check_pair(const Image *src, const Image *dst) {
       dst->format != OVRFSR_FORMAT_RGBA32F)
     return OVRFSR_ERR_UNSUPPORTED; /* UNORM targets follow DetermineOutputFormat: 10-bit in <-> 10-bit out */
   return OVRFSR_OK;
+}
+
+// one image of a stateless NIS dispatch (dst: it is written).  Unlike check_pair, it refuses a format or multisampling
+// before it looks at the pitch.
+static int check_nis_image(const Image *im, bool isDst) {
+  if (!im || !im->data || im->width == 0 || im->height == 0) return OVRFSR_ERR_INVALID;
+  if (im->format < OVRFSR_FORMAT_RGBA8 || im->format > OVRFSR_FORMAT_BGRX8) return OVRFSR_ERR_UNSUPPORTED; /* RGB32F: expand first */
+  if ((isDst && (im->format == OVRFSR_FORMAT_BGRA8 || im->format == OVRFSR_FORMAT_BGRX8)) || im->sample_count > 1) return OVRFSR_ERR_UNSUPPORTED;
+  if (im->array) return validate_array(*im, isDst);
+  const uint32_t bpp = bytes_per_pixel(im->format);
+  if (im->pitch < im->width * bpp || im->pitch % bpp || reinterpret_cast<uintptr_t>(im->data) % bpp) return OVRFSR_ERR_INVALID;
+  return OVRFSR_OK;
+}
+
+// the pass flags of a stateless dispatch: OVRFSR_OK, or the status to return (checked after the images)
+static int check_pass_flags(const Image *src, int pass_flags) {
+  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT)) return OVRFSR_ERR_INVALID;
+  if (pass_flags && src->format != OVRFSR_FORMAT_RGBA16F && src->format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
+  return OVRFSR_OK;
+}
+
+// the status of a stateless dispatch's launch.  cudaErrorInvalidValue is a shape or format the pass does not cover; so
+// is cudaErrorInvalidConfiguration where `configUnsupported` (EASU, fused and NIS refuse a scale with it).  RCAS and
+// CAS refuse nothing with it, so there it is a failed launch.
+static int launch_status(cudaError_t e, bool configUnsupported) {
+  if (e == cudaErrorInvalidValue || (configUnsupported && e == cudaErrorInvalidConfiguration)) return OVRFSR_ERR_UNSUPPORTED;
+  return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
 }
 
 // the two images of a stateless dispatch, untagged; null where the caller passed null
@@ -865,13 +889,6 @@ int ovrfsr_dispatch_fsr_easu(const ovrfsr_image *src_tagged, const ovrfsr_image 
   return ovrfsr_dispatch_fsr_easu_ex(src_tagged, dst_tagged, consts, math_mode, 0, stream);
 }
 
-// the pass flags of a stateless FSR dispatch: OVRFSR_OK, or the status to return (checked after the image pair)
-static int check_pass_flags(const Image *src, int pass_flags) {
-  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT)) return OVRFSR_ERR_INVALID;
-  if (pass_flags && src->format != OVRFSR_FORMAT_RGBA16F && src->format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
-  return OVRFSR_OK;
-}
-
 int ovrfsr_dispatch_fsr_easu_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t consts[24], int math_mode,
                                 int pass_flags, void *stream) {
   const DispatchPair io(src_tagged, dst_tagged);
@@ -879,11 +896,9 @@ int ovrfsr_dispatch_fsr_easu_ex(const ovrfsr_image *src_tagged, const ovrfsr_ima
   if (!consts) return OVRFSR_ERR_INVALID;
   int rc = check_pair(src, dst);
   if (rc != OVRFSR_OK || (rc = check_pass_flags(src, pass_flags)) != OVRFSR_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_easu_strict(pass_image(*src), pass_image(*dst), consts, s, nullptr, 1.0f, nullptr, pass_flags)
-                                                  : launch_easu_fast(pass_image(*src), pass_image(*dst), consts, s, nullptr, 1.0f, nullptr, pass_flags);
-  if (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) return OVRFSR_ERR_UNSUPPORTED;
-  return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
+  return launch_status(launchers(math_mode).easu(pass_image(*src), pass_image(*dst), consts, static_cast<cudaStream_t>(stream), nullptr,
+                                                 1.0f, nullptr, pass_flags),
+                       /*configUnsupported=*/true);
 }
 
 int ovrfsr_dispatch_fsr_fused(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t upscale_consts[24],
@@ -894,12 +909,9 @@ int ovrfsr_dispatch_fsr_fused(const ovrfsr_image *src_tagged, const ovrfsr_image
   if (io.any_array()) return OVRFSR_ERR_UNSUPPORTED; /* the fused kernel has no array I/O */
   int rc = check_pair(src, dst);
   if (rc != OVRFSR_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = math_mode == OVRFSR_MATH_STRICT
-                      ? launch_fsr_fused_strict(pass_image(*src), pass_image(*dst), upscale_consts, sharpen_consts, s)
-                      : launch_fsr_fused_fast(pass_image(*src), pass_image(*dst), upscale_consts, sharpen_consts, s);
-  if (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) return OVRFSR_ERR_UNSUPPORTED;
-  return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
+  return launch_status(launchers(math_mode).fsr_fused(pass_image(*src), pass_image(*dst), upscale_consts, sharpen_consts,
+                                                      static_cast<cudaStream_t>(stream), nullptr),
+                       /*configUnsupported=*/true);
 }
 
 int ovrfsr_dispatch_fsr_rcas(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const uint32_t consts[12], int math_mode,
@@ -915,11 +927,45 @@ int ovrfsr_dispatch_fsr_rcas_ex(const ovrfsr_image *src_tagged, const ovrfsr_ima
   int rc = check_pair(src, dst);
   if (rc != OVRFSR_OK || (rc = check_pass_flags(src, pass_flags)) != OVRFSR_OK) return rc;
   if (src->width != dst->width || src->height != dst->height) return OVRFSR_ERR_INVALID;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_rcas_strict(pass_image(*src), pass_image(*dst), consts, s, false, nullptr, pass_flags)
-                                                  : launch_rcas_fast(pass_image(*src), pass_image(*dst), consts, s, false, nullptr, pass_flags);
-  if (e == cudaErrorInvalidValue) return OVRFSR_ERR_UNSUPPORTED;
-  return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
+  return launch_status(launchers(math_mode).rcas(pass_image(*src), pass_image(*dst), consts, static_cast<cudaStream_t>(stream), false,
+                                                 nullptr, pass_flags),
+                       /*configUnsupported=*/false);
+}
+
+int ovrfsr_dispatch_nis_scaler(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                               void *stream) {
+  return ovrfsr_dispatch_nis_scaler_ex(src_tagged, dst_tagged, cfg256, math_mode, 0, stream);
+}
+
+int ovrfsr_dispatch_nis_sharpen(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                                void *stream) {
+  return ovrfsr_dispatch_nis_sharpen_ex(src_tagged, dst_tagged, cfg256, math_mode, 0, stream);
+}
+
+// NVScaler, or NVSharpen (sharpen), with this library's filter banks
+static int dispatch_nis(bool sharpen, const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                        int pass_flags, void *stream) {
+  const DispatchPair io(src_tagged, dst_tagged);
+  const Image *src = io.src, *dst = io.dst;
+  if (!cfg256) return OVRFSR_ERR_INVALID;
+  int rc = check_nis_image(src, false);
+  if (rc != OVRFSR_OK || (rc = check_nis_image(dst, true)) != OVRFSR_OK) return rc;
+  if ((rc = check_pass_flags(src, pass_flags)) != OVRFSR_OK) return rc;
+  if (sharpen && (src->width != dst->width || src->height != dst->height)) return OVRFSR_ERR_INVALID;
+  const Launchers &L = launchers(math_mode);
+  return launch_status((sharpen ? L.nis_sharpen : L.nis_scaler)(pass_image(*src), pass_image(*dst), cfg256, static_cast<cudaStream_t>(stream),
+                                                                nullptr, pass_flags),
+                       /*configUnsupported=*/true);
+}
+
+int ovrfsr_dispatch_nis_scaler_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                                  int pass_flags, void *stream) {
+  return dispatch_nis(false, src_tagged, dst_tagged, cfg256, math_mode, pass_flags, stream);
+}
+
+int ovrfsr_dispatch_nis_sharpen_ex(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_tagged, const void *cfg256, int math_mode,
+                                   int pass_flags, void *stream) {
+  return dispatch_nis(true, src_tagged, dst_tagged, cfg256, math_mode, pass_flags, stream);
 }
 
 // ---- host constants -----------------------------------------------------------------------------
@@ -965,11 +1011,8 @@ int ovrfsr_dispatch_cas(const ovrfsr_image *src_tagged, const ovrfsr_image *dst_
   if (io.any_array()) return OVRFSR_ERR_UNSUPPORTED; /* CAS has no array I/O */
   int rc = check_pair(src, dst);
   if (rc != OVRFSR_OK) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  cudaError_t e = math_mode == OVRFSR_MATH_STRICT ? launch_cas_strict(pass_image(*src), pass_image(*dst), consts, sharpen_only, s)
-                                                  : launch_cas_fast(pass_image(*src), pass_image(*dst), consts, sharpen_only, s);
-  if (e == cudaErrorInvalidValue) return OVRFSR_ERR_UNSUPPORTED;
-  return e == cudaSuccess ? OVRFSR_OK : OVRFSR_ERR_CUDA;
+  return launch_status(launchers(math_mode).cas(pass_image(*src), pass_image(*dst), consts, sharpen_only, static_cast<cudaStream_t>(stream)),
+                       /*configUnsupported=*/false);
 }
 
 int ovrfsr_selftest_rcp(uint32_t *mismatches, uint32_t *checked) {

@@ -83,5 +83,9 @@ inline bool make_nis_config(NisConfig &c, const ovrfsr_config &cfg, bool sharpen
   return ok;
 }
 
+// NVScaler's filter banks (NIS_Config.h:261-393), float[2][64 * 8]: coef_scale, then coef_usm, each 64 phases x
+// kFilterSize (8) taps, 6 used.  Built on first use (nis_capi.cu).
+const float *nis_coef_banks();
+
 } // namespace host
 } // namespace ovrfsr
