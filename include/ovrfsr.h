@@ -300,7 +300,8 @@ OVRFSR_API int ovrfsr_dispatch_fsr_rcas_ex(const ovrfsr_image *src, const ovrfsr
  * upscaled image is quantised to dst->format (RGBA8, or RGB10A2 for an RGB10A2 source) exactly as the first dispatch
  * stores it, but never leaves shared memory.  Bit-identical to the two dispatches above run back to back.  The two
  * constant blocks must carry the same centres / radius words (they do when built by ovrfsr_make_*_constants for one
- * eye); OVRFSR_ERR_UNSUPPORTED if this pair cannot be fused (formats, out->in scale above ~1.05). */
+ * eye); OVRFSR_ERR_UNSUPPORTED if this pair cannot be fused (formats, or a source
+ * tile beyond the kernel's shared memory: out->in steps above about 0.85 in both axes, above about 1.03 in one). */
 OVRFSR_API int ovrfsr_dispatch_fsr_fused(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t upscale_consts[24],
                                          const uint32_t sharpen_consts[12], int math_mode, void *stream);
 /* g_NISUpscaleShader / g_NISSharpenShader: cfg = NISConfig, 256 bytes (NIS_Config.h:37-77 + the
