@@ -1,5 +1,5 @@
-// minmax_probe.cu -- what sm_90a's fminf / fmaxf / __saturatef return on signed zeros, subnormals, large finite values
-// and NaN, in the two-operand form and in the nested forms the filters use.  tests/test_gpu_minmax_rule.py builds it
+// minmax_probe.cu -- what sm_90a's fminf / fmaxf / __saturatef return on signed zeros, subnormals, large finite values,
+// infinities and NaNs (quiet and signalling, with payloads, of both signs), in the two-operand form and in the nested forms the filters use.  tests/test_gpu_minmax_rule.py builds it
 // twice (-fmad=false / -fmad=true), runs each build once and compares every line with the checker's helpers.
 //
 // The operands are read from device memory, so nothing is folded at compile time: each result is what FMNMX (and the
@@ -10,9 +10,12 @@
 
 #include <cuda_runtime.h>
 
-// {+0, -0, +1, -1, +2^-149, -2^-149, +65504, -65504, NaN}
+// {+0, -0, +1, -1, +2^-149, -2^-149, +65504, -65504, NaN, +inf, -inf, signalling NaNs 0x7f800001 / 0xff800001, quiet
+// NaNs with a payload 0x7fc00001 / with the sign 0xffc00000}: an FP32 eye texture can hold any of them, and RCAS feeds
+// the raw texel to FMNMX
 static const uint32_t kValues[] = {0x00000000u, 0x80000000u, 0x3f800000u, 0xbf800000u, 0x00000001u,
-                                   0x80000001u, 0x477fe000u, 0xc77fe000u, 0x7fc00000u};
+                                   0x80000001u, 0x477fe000u, 0xc77fe000u, 0x7fc00000u, 0x7f800000u,
+                                   0xff800000u, 0x7f800001u, 0xff800001u, 0x7fc00001u, 0xffc00000u};
 constexpr int N = sizeof(kValues) / sizeof(kValues[0]);
 
 // forms, by index into the operand table:
@@ -83,7 +86,7 @@ int main() {
     return 1;
   float *oPairs = dout, *oSat = oPairs + 2 * kPairs, *oTriples = oSat + N, *oQuads = oTriples + 6 * kTriples,
         *oSatForms = oQuads + 2 * kQuads;
-  probe_pairs<<<1, 128>>>(dv, oPairs);
+  probe_pairs<<<(kPairs + 127) / 128, 128>>>(dv, oPairs);
   probe_sat<<<1, 32>>>(dv, oSat);
   probe_triples<<<(kTriples + 255) / 256, 256>>>(dv, oTriples);
   probe_quads<<<(kQuads + 255) / 256, 256>>>(dv, oQuads);

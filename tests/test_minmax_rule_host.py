@@ -4,7 +4,7 @@ D3D11 leaves the sign of min(+0, -0) / max(+0, -0) to the implementation and C l
 returns the first operand), so the checker states its own rule (oracle/ovr_glue.h): NaN-ignoring, -0 < +0, independent
 of operand order -- IEEE 754-2019 minimumNumber / maximumNumber, what sm_90a's FMNMX computes
 (tests/test_gpu_minmax_rule.py).  Here: the exported helpers against a plain statement of that rule on every ordered
-pair of {+-0, +-1, +-2^-149, +-65504, NaN}; the reference shims' min / max / clamp / saturate (oracle/ref_shim) compiled
+pair of {+-0, +-1, +-2^-149, +-65504, +-inf, NaNs of both signs, quiet and signalling, with payloads}; the reference shims' min / max / clamp / saturate (oracle/ref_shim) compiled
 on their own and compared with the helpers; no libm min / max left in the checker's sources."""
 import ctypes as C
 import math
@@ -17,7 +17,12 @@ import numpy as np
 import pytest
 
 ROOT = Path(__file__).resolve().parents[1]
-VALUES = [0.0, -0.0, 1.0, -1.0, 2.0 ** -149, -(2.0 ** -149), 65504.0, -65504.0, math.nan]
+# the operands of tests/cuda/minmax_probe.cu, in its order: +-0, +-1, +-2^-149, +-65504, NaN, +-inf, and the NaNs
+# 0x7f800001 / 0xff800001 (signalling), 0x7fc00001, 0xffc00000.  A Python float cannot carry a signalling float32 NaN
+# (the conversion quietens it), so here they are NaNs like the others; the device probe reads their exact bits.
+NAN_BITS = (0x7f800001, 0xff800001, 0x7fc00001, 0xffc00000)
+VALUES = [0.0, -0.0, 1.0, -1.0, 2.0 ** -149, -(2.0 ** -149), 65504.0, -65504.0, math.nan, math.inf, -math.inf] + \
+    [float(np.uint32(b).view(np.float32)) for b in NAN_BITS]
 
 
 def rule_min(a, b):
@@ -59,6 +64,8 @@ def test_rule_statement_is_order_independent_and_ignores_nan():
                 assert not math.isnan(rule_min(a, b)) and not math.isnan(rule_max(a, b))
     assert bits(rule_min(0.0, -0.0)) == 0x80000000 and bits(rule_max(-0.0, 0.0)) == 0
     assert bits(rule_sat(-0.0)) == 0 and bits(rule_sat(math.nan)) == 0
+    assert bits(rule_sat(math.inf)) == 0x3f800000 and bits(rule_sat(-math.inf)) == 0
+    assert rule_min(math.nan, -math.inf) == -math.inf and rule_max(math.inf, math.nan) == math.inf
 
 
 def test_checker_helpers_follow_the_rule_on_every_pair():
