@@ -168,6 +168,21 @@ typedef struct ovrfsr_config {
  * a config with both bits tone-maps whichever path runs (a host with a use_nis toggle).  This is not the NIS SDK's
  * NIS_HDR_MODE_LINEAR / _PQ.  Changing the bit through ovrfsr_set_config resets the ctx like any config change. */
 #define OVRFSR_FLAG_SRTM_NIS 4
+/* Keep infinities and NaNs of float eye textures out of every pass and every stored pixel, an extension the reference
+ * never enables.  An R16G16B16A16_FLOAT render target overflows to +-inf at 65520, one bad shader pixel can be NaN, and
+ * the filters multiply every texel they read by its weight (inf x 0 = NaN), so one such texel can blacken a UNORM
+ * output pixel or reach the compositor as NaN in a float one.  With this bit, on the FSR and NIS paths with a float
+ * source (RGBA16F, RGBA32F, RGB32F after its expansion, a multisampled one after its resolve):
+ *   finite-in   every channel of every texel a pass decodes: NaN -> +0, +-inf -> +-65504 (the largest RGBA16F value);
+ *               every finite value is kept bit for bit, FP32 values beyond 65504 included.  Before F of the tone map.
+ *   finite-out  every channel of every pixel a pass stores into a float image, the ctx's intermediate included:
+ *               NaN -> +0, clamped to +-65504 (RGBA16F, then rounded) or +-FLT_MAX (RGBA32F).  After G of the tone map.
+ * UNORM stores are unchanged (saturate already maps NaN to 0).  The passes, the intermediate's format, the pairing and
+ * OVRFSR_FLAG_FUSED_FSR are exactly those of the bit clear; the MSAA resolve and the RGB32F expansion are not changed.
+ * Ignored -- same output bits as with the bit clear -- for UNORM sources; on content without infinities or NaNs whose
+ * outputs fit the destination it gives the bits of the bit clear too.  Not a repair: a bad texel still weighs in as 0 or
+ * 65504, not as its neighbours.  Changing the bit through ovrfsr_set_config resets the ctx like any config change. */
+#define OVRFSR_FLAG_FINITE 8
 
 typedef struct ovrfsr_ctx ovrfsr_ctx;
 
@@ -292,6 +307,13 @@ OVRFSR_API int ovrfsr_dispatch_fsr_rcas(const ovrfsr_image *src, const ovrfsr_im
  * either bit with a UNORM source, OVRFSR_ERR_INVALID for unknown bits. */
 #define OVRFSR_PASS_SRTM_IN 1
 #define OVRFSR_PASS_SRTM_OUT 2
+/* finite-in / finite-out of OVRFSR_FLAG_FINITE on the texels the pass reads / the pixels it stores, OR-ed with the SRTM
+ * bits above (read: finite-in before F; store: G before finite-out) and accepted by all four _ex dispatches with the
+ * same errors.  The ctx runs EASU with both, RCAS with both when its source is a float image, NVScaler / NVSharpen with
+ * both, and the fused kernel (no stateless bits) with finite-in.  4 and 8 stay unknown bits (OVRFSR_ERR_INVALID), as
+ * they were before these two existed. */
+#define OVRFSR_PASS_FINITE_IN 16
+#define OVRFSR_PASS_FINITE_OUT 32
 OVRFSR_API int ovrfsr_dispatch_fsr_easu_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[24],
                                            int math_mode, int pass_flags, void *stream);
 OVRFSR_API int ovrfsr_dispatch_fsr_rcas_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[12],
@@ -310,7 +332,8 @@ OVRFSR_API int ovrfsr_dispatch_nis_scaler(const ovrfsr_image *src, const ovrfsr_
                                           int math_mode, void *stream);
 OVRFSR_API int ovrfsr_dispatch_nis_sharpen(const ovrfsr_image *src, const ovrfsr_image *dst, const void *cfg256,
                                            int math_mode, void *stream);
-/* The two NIS dispatches above with the tone map of OVRFSR_FLAG_SRTM_NIS (pass_flags, OR of OVRFSR_PASS_SRTM_IN / _OUT):
+/* The two NIS dispatches above with the tone map of OVRFSR_FLAG_SRTM_NIS (pass_flags, OR of OVRFSR_PASS_SRTM_IN / _OUT,
+ * and of OVRFSR_PASS_FINITE_IN / _OUT):
  * F after the decode of every texel the pass reads, G before the encode of every pixel it stores.  The ctx runs its one
  * NIS pass with both bits.  pass_flags == 0 launches exactly what ovrfsr_dispatch_nis_scaler / _sharpen launch.
  * OVRFSR_ERR_UNSUPPORTED for either bit with a UNORM source, OVRFSR_ERR_INVALID for unknown bits. */

@@ -141,8 +141,9 @@ struct Plan {
   // (apply_post_process), so an update that lands between the two launches cannot split them.
   bool paired = false;
   bool tryFused = false;          // paired and OVRFSR_FLAG_FUSED_FSR: one fused kernel, where the images allow it
-  int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* of each FSR pass
-  int nisSrtm = 0;                // OVRFSR_PASS_SRTM_* of the NIS pass
+  int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* | OVRFSR_PASS_FINITE_* of each FSR pass
+  int nisSrtm = 0;                // OVRFSR_PASS_SRTM_* | OVRFSR_PASS_FINITE_* of the NIS pass
+  int fusedFinite = 0;            // OVRFSR_PASS_FINITE_IN of the fused kernel
   int midFormat = OVRFSR_FORMAT_RGBA8; // of FSR's upscaled image
 };
 
@@ -324,6 +325,19 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
   // amplifies by up to 32768 near 1, so the intermediate keeps them as RGBA32F for a float output, and as RGBA16F for a
   // UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).
   p.midFormat = !srtm ? c->outFormat : (unormOut ? OVRFSR_FORMAT_RGBA16F : OVRFSR_FORMAT_RGBA32F);
+  // OVRFSR_FLAG_FINITE changes no pass and no format, only each pass's bits: finite-in on every pass that reads a float
+  // image, finite-out on every pass that stores one (a UNORM store ignores it, so EASU and NIS always get both).  RCAS
+  // reads the float eye when it runs alone, and EASU's intermediate when that is a float image (a float output, or SRTM);
+  // the paired RCAS reads a UNORM intermediate.  The fused kernel reads the eye and stores UNORM.
+  p.fusedFinite = 0;
+  if ((c->cfg.flags & OVRFSR_FLAG_FINITE) && floatSrc) {
+    const int both = OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_FINITE_OUT;
+    const bool rcasFloatSrc = !p.upscale || p.midFormat == OVRFSR_FORMAT_RGBA16F || p.midFormat == OVRFSR_FORMAT_RGBA32F;
+    p.easuSrtm |= both;
+    p.rcasSrtm |= rcasFloatSrc ? both : 0;
+    p.nisSrtm |= both;
+    p.fusedFinite = OVRFSR_PASS_FINITE_IN;
+  }
   const bool one = c->textureContainsOnlyOneEye;
   const int neyes = one ? 2 : 1;
   for (int e = 0; e < neyes; ++e) {
@@ -445,7 +459,7 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
   // the fused kernel has no array I/O: with an array source or destination the two dispatches run
   if (p.tryFused && !src->array && !fin.array) {
     // EASU and RCAS as one kernel; shapes it does not cover take the two dispatches below
-    e = L.fsr_fused(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev);
+    e = L.fsr_fused(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev, p.fusedFinite);
     if (e == cudaSuccess) fused = true;
     else if (e != cudaErrorInvalidValue && e != cudaErrorInvalidConfiguration) return fail(c, OVRFSR_ERR_CUDA, "fused EASU+RCAS launch", e);
   }
@@ -860,7 +874,8 @@ static int check_nis_image(const Image *im, bool isDst) {
 
 // the pass flags of a stateless dispatch: OVRFSR_OK, or the status to return (checked after the images)
 static int check_pass_flags(const Image *src, int pass_flags) {
-  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT)) return OVRFSR_ERR_INVALID;
+  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT | OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_FINITE_OUT))
+    return OVRFSR_ERR_INVALID;
   if (pass_flags && src->format != OVRFSR_FORMAT_RGBA16F && src->format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
   return OVRFSR_OK;
 }
@@ -910,7 +925,7 @@ int ovrfsr_dispatch_fsr_fused(const ovrfsr_image *src_tagged, const ovrfsr_image
   int rc = check_pair(src, dst);
   if (rc != OVRFSR_OK) return rc;
   return launch_status(launchers(math_mode).fsr_fused(pass_image(*src), pass_image(*dst), upscale_consts, sharpen_consts,
-                                                      static_cast<cudaStream_t>(stream), nullptr),
+                                                      static_cast<cudaStream_t>(stream), nullptr, 0),
                        /*configUnsupported=*/true);
 }
 

@@ -44,6 +44,7 @@ struct FusedArgs {
   float sharp;        // RCAS const0[0]
   float tintGB;       // 1 - debug*0.3
   int vecStore;       // dst base and pitch are 16-byte aligned: 128-bit stores allowed
+  int finiteIn;       // float sources only: finite_in on every texel read (OVRFSR_FLAG_FINITE; the target is UNORM)
 };
 
 template <int FIN, int FMID, int FOUT, int TW, bool TMA>
@@ -144,6 +145,9 @@ __global__ void __launch_bounds__(kThreads, 2) fsr_fused_kernel(const __grid_con
         for (int tx = lane; tx < cols; tx += 32) {
           const int gx = clampi(tx0 + tx, 0, a.src.w - 1);
           float4 c = fetch_texel<FIN>(row, gx);
+          if constexpr (!packed32(FIN)) {
+            if (a.finiteIn) finite_in(c);
+          }
           sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y);
           c.w = 1.0f;
           sC[ty * TW + tx] = c;

@@ -31,7 +31,8 @@ static ovrfsr_config config_from_singleton() {
   for (int i = 0; i < 4; ++i) k.proj_centre[i] = c.projCentre[i];
   k.device = c.cudaDevice;
   k.math_mode = c.strictMath ? OVRFSR_MATH_STRICT : OVRFSR_MATH_FAST;
-  k.flags = (c.fusedFsr ? OVRFSR_FLAG_FUSED_FSR : 0) | (c.srtm ? OVRFSR_FLAG_SRTM : 0) | (c.srtmNis ? OVRFSR_FLAG_SRTM_NIS : 0);
+  k.flags = (c.fusedFsr ? OVRFSR_FLAG_FUSED_FSR : 0) | (c.srtm ? OVRFSR_FLAG_SRTM : 0) | (c.srtmNis ? OVRFSR_FLAG_SRTM_NIS : 0) |
+            (c.finite ? OVRFSR_FLAG_FINITE : 0);
   return k;
 }
 
