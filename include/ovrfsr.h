@@ -183,6 +183,27 @@ typedef struct ovrfsr_config {
  * outputs fit the destination it gives the bits of the bit clear too.  Not a repair: a bad texel still weighs in as 0 or
  * 65504, not as its neighbours.  Changing the bit through ovrfsr_set_config resets the ctx like any config change. */
 #define OVRFSR_FLAG_FINITE 8
+/* Filter linear float eye textures in a perceptual space, and store 8-bit outputs sRGB-encoded, an extension the
+ * reference never enables.  EASU's edge analysis, RCAS's limiter and the NIS thresholds and limits are tuned for
+ * gamma-encoded values, which the reference only feeds them for an 8-bit sRGB eye; and a linear value stored as plain
+ * UNORM8 reads as dark and banded where the compositor takes the 8-bit output as sRGB.  With this bit, on the FSR and
+ * NIS paths with a float source (RGBA16F, RGBA32F, RGB32F after its expansion, a multisampled one after its resolve):
+ *   perceptual-in   every texel a pass decodes, after finite-in and F of the tone map: P(c) = copysign(sqrt(|c|), c)
+ *                   on R, G and B (gamma 2.0, extended to negative channels by sign).
+ *   perceptual-out  every pixel a pass stores, before G of the tone map: c * |c| on R, G and B.  A UNORM8 store then
+ *                   sRGB-encodes the linear value v: code(v) = the number of k in 1..255 with v >= T[k], T[k] the
+ *                   smallest binary32 at or above srgb_to_linear((k - 0.5) / 255) (D3D11's FLOAT -> SRGB conversion
+ *                   without its 0.6-ulp slack; NaN and v <= 0 give 0).  Float stores keep the linear value.
+ * Alpha is untouched.  sqrt and the product are correctly rounded in both math modes, so the maps are bit-exact.
+ * FSR runs without the pairing and OVRFSR_FLAG_FUSED_FSR: EASU stores perceptual values into an RGBA16F intermediate
+ * (RGBA32F for a float output) and RCAS maps them back; RCAS alone runs both maps, and so does the NIS pass.  The
+ * outside-radius copies become encode(G(P^-1(tint x P(F(c))))): close to a copy, not bit-exact.  When the last pass
+ * sRGB-encodes (an RGBA8 output), the image ovrfsr_apply / ovrfsr_apply_pair return carries OVRFSR_FORMAT_SRGB_BIT,
+ * and ovrfsr_apply_into / _pair_into accept a destination of the output format with or without that tag.  Negative,
+ * NaN and infinite channels get whatever IEEE arithmetic gives (OVRFSR_FLAG_FINITE keeps the last two out).  Ignored --
+ * same output bits as with the bit clear -- for UNORM sources.  Changing the bit through ovrfsr_set_config resets the
+ * ctx like any config change. */
+#define OVRFSR_FLAG_PERCEPTUAL 16
 
 typedef struct ovrfsr_ctx ovrfsr_ctx;
 
@@ -207,7 +228,10 @@ OVRFSR_API int ovrfsr_get_config(const ovrfsr_ctx *ctx, ovrfsr_config *cfg);
  *   only_one_eye  |uMax-uMin| > .5 of the submit bounds (:146); 0 = both eyes side by side in src
  *   out           receives the ctx-owned output image (upscaled+sharpened); valid until the next
  *                 apply for the same eye, reset or destroy.  One output per eye (the reference
- *                 shares one between both eyes, PostProcessor.h:43,58).
+ *                 shares one between both eyes, PostProcessor.h:43,58).  Its format carries
+ *                 OVRFSR_FORMAT_SRGB_BIT when the output is sRGB-encoded (OVRFSR_FLAG_PERCEPTUAL); it can be passed
+ *                 back as a source as it is, but a host that passes it as a destination (ovrfsr_image_copy, a
+ *                 dispatch) clears the tag first.
  *   stream        cudaStream_t; work is enqueued asynchronously, nothing is synchronised.  The ctx reuses its per-eye
  *                 intermediates and outputs on every call, so successive calls for the SAME eye of one ctx must be
  *                 ordered (same stream, or the caller's own events); the two eyes may run on different streams, and
@@ -314,6 +338,12 @@ OVRFSR_API int ovrfsr_dispatch_fsr_rcas(const ovrfsr_image *src, const ovrfsr_im
  * they were before these two existed. */
 #define OVRFSR_PASS_FINITE_IN 16
 #define OVRFSR_PASS_FINITE_OUT 32
+/* perceptual-in / perceptual-out of OVRFSR_FLAG_PERCEPTUAL on the texels the pass reads / the pixels it stores, OR-ed
+ * with the bits above (read: finite-in, F, then P; store: P^-1, G, then finite-out or the sRGB encode of an RGBA8 target)
+ * and accepted by all four _ex dispatches with the same errors.  The ctx runs EASU with _IN, RCAS with _OUT after EASU
+ * and with both alone, NVScaler / NVSharpen with both.  4, 8, 64 and 256 stay unknown bits (OVRFSR_ERR_INVALID). */
+#define OVRFSR_PASS_PERCEPTUAL_IN 128
+#define OVRFSR_PASS_PERCEPTUAL_OUT 512
 OVRFSR_API int ovrfsr_dispatch_fsr_easu_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[24],
                                            int math_mode, int pass_flags, void *stream);
 OVRFSR_API int ovrfsr_dispatch_fsr_rcas_ex(const ovrfsr_image *src, const ovrfsr_image *dst, const uint32_t consts[12],

@@ -21,8 +21,10 @@ FLAG_FUSED_FSR = 1
 FLAG_SRTM = 2  # AMD's reversible tone map around the FSR passes of a float source
 FLAG_SRTM_NIS = 4  # the same tone map around the NIS pass of a float source
 FLAG_FINITE = 8  # no infinity or NaN of a float source enters a pass or a stored float pixel
+FLAG_PERCEPTUAL = 16  # a float source is filtered as gamma 2.0, and an RGBA8 output stores sRGB codes
 PASS_SRTM_IN, PASS_SRTM_OUT = 1, 2  # pass_flags of ovrfsr_dispatch_{fsr_easu,fsr_rcas,nis_scaler,nis_sharpen}_ex
 PASS_FINITE_IN, PASS_FINITE_OUT = 16, 32  # OR-ed with the SRTM bits: finite-in on the texels read, finite-out on the pixels stored
+PASS_PERCEPTUAL_IN, PASS_PERCEPTUAL_OUT = 128, 512  # OR-ed with the above: P on the texels read, P^-1 (and the sRGB encode) on the pixels stored
 
 
 class Image(C.Structure):

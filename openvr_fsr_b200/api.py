@@ -32,6 +32,7 @@ class Config:
     srtm: bool = False      # OVRFSR_FLAG_SRTM: FSR on a float (HDR) source runs between AMD's reversible tone map and its inverse
     srtmNis: bool = False   # OVRFSR_FLAG_SRTM_NIS: NIS on a float (HDR) source runs between the same tone map and its inverse
     finite: bool = False    # OVRFSR_FLAG_FINITE: no infinity or NaN of a float source enters a pass or a stored float pixel
+    perceptual: bool = False  # OVRFSR_FLAG_PERCEPTUAL: a float source is filtered as gamma 2.0, an RGBA8 output is sRGB-encoded
 
     def to_c(self) -> L.Config:
         c = L.Config()
@@ -42,7 +43,8 @@ class Config:
         c.proj_centre = (C.c_float * 4)(*self.projCentre)
         c.device, c.output_format, c.math_mode = self.device, self.outputFormat, self.mathMode
         c.flags = (L.FLAG_FUSED_FSR if self.fusedFsr else 0) | (L.FLAG_SRTM if self.srtm else 0) | \
-            (L.FLAG_SRTM_NIS if self.srtmNis else 0) | (L.FLAG_FINITE if self.finite else 0)
+            (L.FLAG_SRTM_NIS if self.srtmNis else 0) | (L.FLAG_FINITE if self.finite else 0) | \
+            (L.FLAG_PERCEPTUAL if self.perceptual else 0)
         return c
 
 
@@ -353,9 +355,10 @@ def _dispatch(fn, src, dst, consts, math_mode, stream, src_fmt=None, dst_fmt=Non
     return dst
 
 
-def _pass_flags(srtm_in, srtm_out, finite_in=False, finite_out=False):
+def _pass_flags(srtm_in, srtm_out, finite_in=False, finite_out=False, perceptual_in=False, perceptual_out=False):
     return (L.PASS_SRTM_IN if srtm_in else 0) | (L.PASS_SRTM_OUT if srtm_out else 0) | \
-        (L.PASS_FINITE_IN if finite_in else 0) | (L.PASS_FINITE_OUT if finite_out else 0)
+        (L.PASS_FINITE_IN if finite_in else 0) | (L.PASS_FINITE_OUT if finite_out else 0) | \
+        (L.PASS_PERCEPTUAL_IN if perceptual_in else 0) | (L.PASS_PERCEPTUAL_OUT if perceptual_out else 0)
 
 
 def _dispatch_ex(fn, src, dst, consts, math_mode, flags, stream, src_fmt=None, dst_fmt=None):
@@ -365,22 +368,23 @@ def _dispatch_ex(fn, src, dst, consts, math_mode, flags, stream, src_fmt=None, d
 
 
 def fsr_easu(src, dst, consts24, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False,
-             finite_in=False, finite_out=False):
+             finite_in=False, finite_out=False, perceptual_in=False, perceptual_out=False):
     """g_FSRUpscaleShader.  srtm_in / srtm_out (float sources only): AMD's reversible tone map on every texel read / its
     inverse on every pixel stored; finite_in / finite_out (float sources only): OVRFSR_FLAG_FINITE's maps on the same
-    texels / pixels (ovrfsr_dispatch_fsr_easu_ex)"""
+    texels / pixels; perceptual_in / perceptual_out (float sources only): OVRFSR_FLAG_PERCEPTUAL's maps, the sRGB encode
+    of an RGBA8 target included (ovrfsr_dispatch_fsr_easu_ex)"""
     c = (C.c_uint32 * 24)(*[int(x) for x in consts24])
-    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out)
+    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out, perceptual_in, perceptual_out)
     if flags:
         return _dispatch_ex(L.lib().ovrfsr_dispatch_fsr_easu_ex, src, dst, c, math_mode, flags, stream, src_fmt, dst_fmt)
     return _dispatch(L.lib().ovrfsr_dispatch_fsr_easu, src, dst, c, math_mode, stream, src_fmt, dst_fmt)
 
 
 def fsr_rcas(src, dst, consts12, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False,
-             finite_in=False, finite_out=False):
-    """g_FSRSharpenShader.  srtm_* / finite_* as for fsr_easu (ovrfsr_dispatch_fsr_rcas_ex)"""
+             finite_in=False, finite_out=False, perceptual_in=False, perceptual_out=False):
+    """g_FSRSharpenShader.  srtm_* / finite_* / perceptual_* as for fsr_easu (ovrfsr_dispatch_fsr_rcas_ex)"""
     c = (C.c_uint32 * 12)(*[int(x) for x in consts12])
-    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out)
+    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out, perceptual_in, perceptual_out)
     if flags:
         return _dispatch_ex(L.lib().ovrfsr_dispatch_fsr_rcas_ex, src, dst, c, math_mode, flags, stream, src_fmt, dst_fmt)
     return _dispatch(L.lib().ovrfsr_dispatch_fsr_rcas, src, dst, c, math_mode, stream, src_fmt, dst_fmt)
@@ -397,12 +401,13 @@ def fsr_fused(src, dst, consts24, consts12, math_mode=L.MATH_STRICT, stream=None
 
 
 def nis_scaler(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False,
-               finite_in=False, finite_out=False):
+               finite_in=False, finite_out=False, perceptual_in=False, perceptual_out=False):
     """g_NISUpscaleShader.  srtm_in / srtm_out (float sources only): AMD's reversible tone map on every texel read / its
     inverse on every pixel stored; finite_in / finite_out (float sources only): OVRFSR_FLAG_FINITE's maps on the same
-    texels / pixels (ovrfsr_dispatch_nis_scaler_ex)"""
+    texels / pixels; perceptual_in / perceptual_out (float sources only): OVRFSR_FLAG_PERCEPTUAL's maps, the sRGB encode
+    of an RGBA8 target included (ovrfsr_dispatch_nis_scaler_ex)"""
     buf = C.create_string_buffer(bytes(cfg256), 256)
-    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out)
+    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out, perceptual_in, perceptual_out)
     if flags:
         return _dispatch_ex(L.lib().ovrfsr_dispatch_nis_scaler_ex, src, dst, C.cast(buf, C.c_void_p), math_mode, flags, stream,
                             src_fmt, dst_fmt)
@@ -410,10 +415,10 @@ def nis_scaler(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_
 
 
 def nis_sharpen(src, dst, cfg256: bytes, math_mode=L.MATH_FAST, stream=None, src_fmt=None, dst_fmt=None, srtm_in=False, srtm_out=False,
-                finite_in=False, finite_out=False):
-    """g_NISSharpenShader.  srtm_* / finite_* as for nis_scaler (ovrfsr_dispatch_nis_sharpen_ex)"""
+                finite_in=False, finite_out=False, perceptual_in=False, perceptual_out=False):
+    """g_NISSharpenShader.  srtm_* / finite_* / perceptual_* as for nis_scaler (ovrfsr_dispatch_nis_sharpen_ex)"""
     buf = C.create_string_buffer(bytes(cfg256), 256)
-    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out)
+    flags = _pass_flags(srtm_in, srtm_out, finite_in, finite_out, perceptual_in, perceptual_out)
     if flags:
         return _dispatch_ex(L.lib().ovrfsr_dispatch_nis_sharpen_ex, src, dst, C.cast(buf, C.c_void_p), math_mode, flags, stream,
                             src_fmt, dst_fmt)

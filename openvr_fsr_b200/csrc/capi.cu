@@ -141,11 +141,23 @@ struct Plan {
   // (apply_post_process), so an update that lands between the two launches cannot split them.
   bool paired = false;
   bool tryFused = false;          // paired and OVRFSR_FLAG_FUSED_FSR: one fused kernel, where the images allow it
-  int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* | OVRFSR_PASS_FINITE_* of each FSR pass
-  int nisSrtm = 0;                // OVRFSR_PASS_SRTM_* | OVRFSR_PASS_FINITE_* of the NIS pass
+  int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* | _FINITE_* | _PERCEPTUAL_* of each FSR pass
+  int nisSrtm = 0;                // OVRFSR_PASS_SRTM_* | _FINITE_* | _PERCEPTUAL_* of the NIS pass
   int fusedFinite = 0;            // OVRFSR_PASS_FINITE_IN of the fused kernel
   int midFormat = OVRFSR_FORMAT_RGBA8; // of FSR's upscaled image
+  bool srgbOut = false;           // the last pass sRGB-encodes its UNORM8 store (OVRFSR_FLAG_PERCEPTUAL)
 };
+
+bool float_source(int format) {
+  return format == OVRFSR_FORMAT_RGBA16F || format == OVRFSR_FORMAT_RGBA32F || format == OVRFSR_FORMAT_RGB32F;
+}
+// OVRFSR_FLAG_PERCEPTUAL with a float source and an RGBA8 output (a float source never gets RGB10A2): the last pass
+// stores sRGB codes.  Decided from the config and the source alone, so that apply_impl can judge a destination's tag
+// before prepare_resources runs.
+bool srgb_output(const ovrfsr_config &cfg, int srcFormat) {
+  return (cfg.flags & OVRFSR_FLAG_PERCEPTUAL) && float_source(srcFormat) &&
+         (cfg.output_format == OVRFSR_FORMAT_AUTO || cfg.output_format == OVRFSR_FORMAT_RGBA8);
+}
 
 } // namespace
 
@@ -311,20 +323,32 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
   // OVRFSR_FLAG_SRTM takes effect on the FSR path with a float source (an RGB32F one is read through its RGBA32F copy, a
   // multisampled one after its resolve), OVRFSR_FLAG_SRTM_NIS on the NIS path with one; UNORM sources are
   // display-referred already
-  const bool floatSrc = src->format == OVRFSR_FORMAT_RGBA16F || src->format == OVRFSR_FORMAT_RGBA32F || src->format == OVRFSR_FORMAT_RGB32F;
+  const bool floatSrc = float_source(src->format);
   const bool srtm = !p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM) && floatSrc;
+  // OVRFSR_FLAG_PERCEPTUAL on either path: the passes filter P(texel), and the last one stores P^-1 of its result
+  const bool perceptual = (c->cfg.flags & OVRFSR_FLAG_PERCEPTUAL) && floatSrc;
   // NIS runs one pass: F on every texel it reads, G on every pixel it stores
   p.nisSrtm = p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM_NIS) && floatSrc ? OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT : 0;
-  p.paired = !p.nis && p.upscale && unormOut && !srtm;
+  p.paired = !p.nis && p.upscale && unormOut && !srtm && !perceptual;
   p.tryFused = p.paired && (c->cfg.flags & OVRFSR_FLAG_FUSED_FSR);
   // SRTM: EASU applies F on read and stores tone-mapped values, RCAS applies G on store, and F on read too when it is
   // the only pass
   p.easuSrtm = srtm ? OVRFSR_PASS_SRTM_IN : 0;
   p.rcasSrtm = !srtm ? 0 : OVRFSR_PASS_SRTM_OUT | (p.upscale ? 0 : OVRFSR_PASS_SRTM_IN);
+  // PERCEPTUAL the same way: EASU maps on read and stores perceptual values, RCAS maps back on store (and on read when
+  // alone), the NIS pass does both.  Read order finite-in, F, P; store order P^-1, G, finite-out (map_in / map_out).
+  if (perceptual) {
+    p.easuSrtm |= OVRFSR_PASS_PERCEPTUAL_IN;
+    p.rcasSrtm |= OVRFSR_PASS_PERCEPTUAL_OUT | (p.upscale ? 0 : OVRFSR_PASS_PERCEPTUAL_IN);
+    p.nisSrtm |= p.nis ? OVRFSR_PASS_PERCEPTUAL_IN | OVRFSR_PASS_PERCEPTUAL_OUT : 0;
+  }
+  p.srgbOut = srgb_output(c->cfg, src->format);
   // The reference's upscaled image has the output format; with SRTM, EASU stores tone-mapped values that RCAS's G
   // amplifies by up to 32768 near 1, so the intermediate keeps them as RGBA32F for a float output, and as RGBA16F for a
-  // UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).
-  p.midFormat = !srtm ? c->outFormat : (unormOut ? OVRFSR_FORMAT_RGBA16F : OVRFSR_FORMAT_RGBA32F);
+  // UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).  Perceptual
+  // values take the same rule: RCAS's P^-1 squares them, and an RGBA8 intermediate would quantise them like a gamma-2.0
+  // 8-bit image before the sRGB encode.
+  p.midFormat = !srtm && !perceptual ? c->outFormat : (unormOut ? OVRFSR_FORMAT_RGBA16F : OVRFSR_FORMAT_RGBA32F);
   // OVRFSR_FLAG_FINITE changes no pass and no format, only each pass's bits: finite-in on every pass that reads a float
   // image, finite-out on every pass that stores one (a UNORM store ignores it, so EASU and NIS always get both).  RCAS
   // reads the float eye when it runs alone, and EASU's intermediate when that is a float image (a float output, or SRTM);
@@ -523,6 +547,9 @@ int apply_impl(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *src_tagged, int onl
   Image src_u{}, dst_u{};
   if (src_tagged) src_u = untagged(*src_tagged);
   if (dst_tagged) dst_u = untagged(*dst_tagged, false);
+  // an sRGB-encoded output may be written into an RGBA8 destination tagged as sRGB (what ovrfsr_apply returns for it)
+  if (src_tagged && dst_tagged && dst_u.format == (OVRFSR_FORMAT_RGBA8 | OVRFSR_FORMAT_SRGB_BIT) && srgb_output(ctx->cfg, src_u.format))
+    dst_u.format = OVRFSR_FORMAT_RGBA8;
   const Image *src = src_tagged ? &src_u : nullptr, *dst = dst_tagged ? &dst_u : nullptr;
   // PostProcessor.cpp:124: disabled or unusable texture -> the frame passes through untouched
   if (!ctx->enabled || !ctx->cfg.fsr_enabled) return OVRFSR_PASSTHROUGH;
@@ -552,7 +579,10 @@ int apply_impl(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *src_tagged, int onl
   }
   ctx->lastSubmittedTexture = src->data;
   ctx->eyeCount = (ctx->eyeCount + 1) % 2;
-  if (out) *out = tagged(ctx->lastOutput);
+  if (out) {
+    *out = tagged(ctx->lastOutput);
+    if (ctx->plan.srgbOut) out->format |= OVRFSR_FORMAT_SRGB_BIT;
+  }
   return OVRFSR_OK;
 }
 
@@ -789,7 +819,7 @@ int ovrfsr_apply_host(ovrfsr_ctx *ctx, int eye, const ovrfsr_image *src_tagged, 
   ovrfsr_image out{};
   rc = ovrfsr_apply(ctx, eye, &st.img, only_one_eye, &out, stream);
   if (rc != OVRFSR_OK) return rc;
-  if (dst_host->width != out.width || dst_host->height != out.height || dst_host->format != out.format)
+  if (dst_host->width != out.width || dst_host->height != out.height || dst_host->format != (out.format & ~OVRFSR_FORMAT_SRGB_BIT))
     return fail(ctx, OVRFSR_ERR_INVALID, "host destination does not match the output size/format");
   const size_t outRowBytes = (size_t)out.width * bytes_per_pixel(out.format);
   if (dst_host->pitch == outRowBytes && out.pitch != outRowBytes) {
@@ -874,7 +904,8 @@ static int check_nis_image(const Image *im, bool isDst) {
 
 // the pass flags of a stateless dispatch: OVRFSR_OK, or the status to return (checked after the images)
 static int check_pass_flags(const Image *src, int pass_flags) {
-  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT | OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_FINITE_OUT))
+  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT | OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_FINITE_OUT |
+                     OVRFSR_PASS_PERCEPTUAL_IN | OVRFSR_PASS_PERCEPTUAL_OUT))
     return OVRFSR_ERR_INVALID;
   if (pass_flags && src->format != OVRFSR_FORMAT_RGBA16F && src->format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
   return OVRFSR_OK;

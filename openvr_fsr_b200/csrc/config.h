@@ -21,6 +21,7 @@ struct Config {
   bool srtm = false;        // OVRFSR_FLAG_SRTM: FSR on a float (HDR) eye texture runs inside AMD's reversible tone map
   bool srtmNis = false;     // OVRFSR_FLAG_SRTM_NIS: NIS on a float (HDR) eye texture runs inside the same tone map
   bool finite = false;      // OVRFSR_FLAG_FINITE: no infinity or NaN of a float eye texture enters a pass or a stored pixel
+  bool perceptual = false;  // OVRFSR_FLAG_PERCEPTUAL: a float eye texture is filtered as gamma 2.0, an 8-bit output is sRGB
 
   // ONE instance per process, owned by libovrfsr.so (an inline function-local static would be duplicated in every
   // module that includes this header when the library is built with hidden visibility)

@@ -41,8 +41,8 @@ struct EasuArgs {
   // intermediate `dst` only where an edge-adjacent group is inside the radius (RCAS reads one pixel across the edge).
   ImageRW direct;           // ptr == nullptr: plain dispatch
   float tintGB;             // 1 - debug*0.3 of the following RCAS pass
-  // float sources only, OVRFSR_PASS_* bits (map_in / map_out): srtmIn = SRTM_IN | FINITE_IN on every texel read,
-  // srtmOut = SRTM_OUT | FINITE_OUT on every pixel stored
+  // float sources only, OVRFSR_PASS_* bits (map_in / map_out): srtmIn = SRTM_IN | FINITE_IN | PERCEPTUAL_IN on every
+  // texel read, srtmOut = SRTM_OUT | FINITE_OUT | PERCEPTUAL_OUT on every pixel stored
   int srtmIn, srtmOut;
 };
 
@@ -591,8 +591,8 @@ __global__ void __launch_bounds__(kThreads, easu_min_ctas(TW)) easu_kernel(const
         const int y = yFirst + 2 * k;
         if (y >= a.dst.h) break;
         float3 c = easu_bilinear(sC, TW, ax, sRowAxis[y - oy0]);
-        // SRTM_OUT never comes with `direct` (the launcher rejects SRTM on a paired launch), and FINITE_OUT does nothing
-        // there: `direct` is a UNORM target
+        // SRTM_OUT and PERCEPTUAL_OUT never come with `direct` (the launcher rejects them on a paired launch), and
+        // FINITE_OUT does nothing there: `direct` is a UNORM target
         if constexpr (!packed32(FIN)) map_out<FOUT>(a.srtmOut, c.x, c.y, c.z);
         if (mid) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
         if constexpr (direct) {
@@ -880,7 +880,8 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       const float4 e = p[k * kRcasTW];
       float r = 1.0f * e.x, g = a.tintGB * e.y, bl = a.tintGB * e.z, al = 1.0f * e.w;
       if constexpr (!packed32(FIN)) {
-        // the copy runs in tone-mapped space: G(tint x F(texel)), alpha untouched by G but clamped by finite_out
+        // the copy runs in the mapped space: G(P^-1(tint x P(F(texel)))), alpha untouched by the maps but clamped by
+        // finite_out
         map_out<FOUT>(a.srtmOut, r, g, bl);
         if constexpr (!packed32(FOUT)) {
           if (a.srtmOut & OVRFSR_PASS_FINITE_OUT) al = finite_out<FOUT>(al);

@@ -29,8 +29,8 @@ struct Launchers {
   //   8-9 NISConfig kSharpStrengthMin / kSharpStrengthScale, 10-11 kSharpLimitMin / kSharpLimitScale (NVScaler and
   //   NVSharpen), 7 and 12-15 padding.  EASU reads words 0-5 only.
   // `srtm` (EASU and RCAS): OVRFSR_PASS_SRTM_* bits, AMD's reversible tone map on the texels read / the pixels stored,
-  // OR-ed with OVRFSR_PASS_FINITE_* (OVRFSR_FLAG_FINITE).  Float sources only, and the SRTM bits never together with the
-  // pairing: cudaErrorInvalidValue otherwise.
+  // OR-ed with OVRFSR_PASS_FINITE_* (OVRFSR_FLAG_FINITE) and OVRFSR_PASS_PERCEPTUAL_* (OVRFSR_FLAG_PERCEPTUAL).  Float
+  // sources only, and the SRTM and perceptual bits never together with the pairing: cudaErrorInvalidValue otherwise.
   cudaError_t (*easu)(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,
                       const PassImage *direct, float tintGB, const uint32_t *centreDev, int srtm);
   cudaError_t (*rcas)(const PassImage &src, const PassImage &dst, const uint32_t consts[12], cudaStream_t s,
@@ -42,8 +42,8 @@ struct Launchers {
   cudaError_t (*fsr_fused)(const PassImage &src, const PassImage &dst, const uint32_t ku[24], const uint32_t ks[12],
                            cudaStream_t s, const uint32_t *centreDev, int finite);
   // NIS (nis_kernels.cuh), with this library's filter banks.  cfg256 = the 256-byte NISConfig block.  `srtm`:
-  // OVRFSR_PASS_SRTM_* / _FINITE_* bits as for EASU and RCAS (OVRFSR_FLAG_SRTM_NIS, OVRFSR_FLAG_FINITE).  Float sources
-  // only: cudaErrorInvalidValue otherwise.
+  // OVRFSR_PASS_SRTM_* / _FINITE_* / _PERCEPTUAL_* bits as for EASU and RCAS (OVRFSR_FLAG_SRTM_NIS, OVRFSR_FLAG_FINITE,
+  // OVRFSR_FLAG_PERCEPTUAL).  Float sources only: cudaErrorInvalidValue otherwise.
   cudaError_t (*nis_scaler)(const PassImage &src, const PassImage &dst, const void *cfg256, cudaStream_t s,
                             const uint32_t *centreDev, int srtm);
   cudaError_t (*nis_sharpen)(const PassImage &src, const PassImage &dst, const void *cfg256, cudaStream_t s,

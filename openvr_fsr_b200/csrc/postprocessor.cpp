@@ -32,7 +32,7 @@ static ovrfsr_config config_from_singleton() {
   k.device = c.cudaDevice;
   k.math_mode = c.strictMath ? OVRFSR_MATH_STRICT : OVRFSR_MATH_FAST;
   k.flags = (c.fusedFsr ? OVRFSR_FLAG_FUSED_FSR : 0) | (c.srtm ? OVRFSR_FLAG_SRTM : 0) | (c.srtmNis ? OVRFSR_FLAG_SRTM_NIS : 0) |
-            (c.finite ? OVRFSR_FLAG_FINITE : 0);
+            (c.finite ? OVRFSR_FLAG_FINITE : 0) | (c.perceptual ? OVRFSR_FLAG_PERCEPTUAL : 0);
   return k;
 }
 
@@ -106,7 +106,18 @@ void PostProcessor::Apply(EVREye eEye, const Texture_t *pTexture, const VRTextur
     outputImage[eye] = out;
     const_cast<Texture_t *>(pTexture)->handle = &outputImage[eye];
   }
-  const_cast<Texture_t *>(pTexture)->eColorSpace = inputIsSrgb ? ColorSpace_Gamma : ColorSpace_Auto;
+  // an sRGB-encoded output (OVRFSR_FLAG_PERCEPTUAL on a float eye into an 8-bit output) is gamma whatever the eye was.
+  // The returned image says so with its tag; a caller's target has the ctx's output format, RGBA8 exactly when that is
+  // 8-bit, and its tag is the caller's choice, so the ctx's config decides there.
+  bool srgbOut = (out.format & OVRFSR_FORMAT_SRGB_BIT) != 0;
+  if (target) {
+    ovrfsr_config k{};
+    const int layout = texture->format & OVRFSR_FORMAT_LAYOUT_MASK;
+    const bool floatEye = layout == OVRFSR_FORMAT_RGBA16F || layout == OVRFSR_FORMAT_RGBA32F || layout == OVRFSR_FORMAT_RGB32F;
+    srgbOut = ovrfsr_get_config(ctx, &k) == OVRFSR_OK && (k.flags & OVRFSR_FLAG_PERCEPTUAL) && floatEye &&
+              (lastTarget->format & OVRFSR_FORMAT_LAYOUT_MASK) == OVRFSR_FORMAT_RGBA8;
+  }
+  const_cast<Texture_t *>(pTexture)->eColorSpace = inputIsSrgb || srgbOut ? ColorSpace_Gamma : ColorSpace_Auto;
 }
 
 void PostProcessor::Reset() {
