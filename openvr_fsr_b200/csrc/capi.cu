@@ -15,6 +15,7 @@
 #include "host_constants.h"
 #include "kernels.h"
 #include "nis_host.h"
+#include "plan.h"
 
 namespace ovrfsr {
 static std::atomic<uint64_t> g_launches{0};
@@ -126,38 +127,6 @@ struct Focus {
   // some eye has a focus or a radius override, or the sharpness is overridden: applies copy the slot
   bool any() const { return set[0] || set[1] || radiusSet[0] || radiusSet[1] || sharpSet; }
 };
-
-// What every apply of a context runs (PostProcessor.cpp:586-594), decided by prepare_resources from the config, the
-// source format and the output format, none of which can change before the next prepare_resources.  FSR always runs
-// RCAS, after EASU when upscaling; NIS runs one pass, NVScaler when upscaling and NVSharpen otherwise.  The last pass
-// writes the caller's image or the ctx's output image.
-struct Plan {
-  bool nis = false;
-  bool upscale = false; // render_scale != 1
-  // EASU followed by RCAS with a UNORM target: EASU writes the outside-radius groups straight to the final image and
-  // RCAS only visits what is inside the radius (kernels.h).  The two passes must classify every group the same way, or
-  // a group would be written by neither or filtered twice: with a focus or a radius override both read their centre
-  // and radius words from the one device block that the single copy at the head of the apply wrote on the same stream
-  // (apply_post_process), so an update that lands between the two launches cannot split them.
-  bool paired = false;
-  bool tryFused = false;          // paired and OVRFSR_FLAG_FUSED_FSR: one fused kernel, where the images allow it
-  int easuSrtm = 0, rcasSrtm = 0; // OVRFSR_PASS_SRTM_* | _FINITE_* | _PERCEPTUAL_* of each FSR pass
-  int nisSrtm = 0;                // OVRFSR_PASS_SRTM_* | _FINITE_* | _PERCEPTUAL_* of the NIS pass
-  int fusedFinite = 0;            // OVRFSR_PASS_FINITE_IN of the fused kernel
-  int midFormat = OVRFSR_FORMAT_RGBA8; // of FSR's upscaled image
-  bool srgbOut = false;           // the last pass sRGB-encodes its UNORM8 store (OVRFSR_FLAG_PERCEPTUAL)
-};
-
-bool float_source(int format) {
-  return format == OVRFSR_FORMAT_RGBA16F || format == OVRFSR_FORMAT_RGBA32F || format == OVRFSR_FORMAT_RGB32F;
-}
-// OVRFSR_FLAG_PERCEPTUAL with a float source and an RGBA8 output (a float source never gets RGB10A2): the last pass
-// stores sRGB codes.  Decided from the config and the source alone, so that apply_impl can judge a destination's tag
-// before prepare_resources runs.
-bool srgb_output(const ovrfsr_config &cfg, int srcFormat) {
-  return (cfg.flags & OVRFSR_FLAG_PERCEPTUAL) && float_source(srcFormat) &&
-         (cfg.output_format == OVRFSR_FORMAT_AUTO || cfg.output_format == OVRFSR_FORMAT_RGBA8);
-}
 
 } // namespace
 
@@ -316,52 +285,8 @@ int prepare_resources(ovrfsr_ctx *c, const ovrfsr_image *src) {
       c->outFormat != (tenBit ? OVRFSR_FORMAT_RGB10A2 : OVRFSR_FORMAT_RGBA8))
     return fail(c, OVRFSR_ERR_UNSUPPORTED, tenBit ? "output format for an RGB10A2 source must be RGB10A2, RGBA16F or RGBA32F"
                                                   : "output format must be RGBA8, RGBA16F or RGBA32F");
-  Plan &p = c->plan;
-  p.nis = c->cfg.use_nis != 0;
-  p.upscale = c->cfg.render_scale != 1.f;
-  const bool unormOut = c->outFormat == OVRFSR_FORMAT_RGBA8 || c->outFormat == OVRFSR_FORMAT_RGB10A2;
-  // OVRFSR_FLAG_SRTM takes effect on the FSR path with a float source (an RGB32F one is read through its RGBA32F copy, a
-  // multisampled one after its resolve), OVRFSR_FLAG_SRTM_NIS on the NIS path with one; UNORM sources are
-  // display-referred already
-  const bool floatSrc = float_source(src->format);
-  const bool srtm = !p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM) && floatSrc;
-  // OVRFSR_FLAG_PERCEPTUAL on either path: the passes filter P(texel), and the last one stores P^-1 of its result
-  const bool perceptual = (c->cfg.flags & OVRFSR_FLAG_PERCEPTUAL) && floatSrc;
-  // NIS runs one pass: F on every texel it reads, G on every pixel it stores
-  p.nisSrtm = p.nis && (c->cfg.flags & OVRFSR_FLAG_SRTM_NIS) && floatSrc ? OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT : 0;
-  p.paired = !p.nis && p.upscale && unormOut && !srtm && !perceptual;
-  p.tryFused = p.paired && (c->cfg.flags & OVRFSR_FLAG_FUSED_FSR);
-  // SRTM: EASU applies F on read and stores tone-mapped values, RCAS applies G on store, and F on read too when it is
-  // the only pass
-  p.easuSrtm = srtm ? OVRFSR_PASS_SRTM_IN : 0;
-  p.rcasSrtm = !srtm ? 0 : OVRFSR_PASS_SRTM_OUT | (p.upscale ? 0 : OVRFSR_PASS_SRTM_IN);
-  // PERCEPTUAL the same way: EASU maps on read and stores perceptual values, RCAS maps back on store (and on read when
-  // alone), the NIS pass does both.  Read order finite-in, F, P; store order P^-1, G, finite-out (map_in / map_out).
-  if (perceptual) {
-    p.easuSrtm |= OVRFSR_PASS_PERCEPTUAL_IN;
-    p.rcasSrtm |= OVRFSR_PASS_PERCEPTUAL_OUT | (p.upscale ? 0 : OVRFSR_PASS_PERCEPTUAL_IN);
-    p.nisSrtm |= p.nis ? OVRFSR_PASS_PERCEPTUAL_IN | OVRFSR_PASS_PERCEPTUAL_OUT : 0;
-  }
-  p.srgbOut = srgb_output(c->cfg, src->format);
-  // The reference's upscaled image has the output format; with SRTM, EASU stores tone-mapped values that RCAS's G
-  // amplifies by up to 32768 near 1, so the intermediate keeps them as RGBA32F for a float output, and as RGBA16F for a
-  // UNORM output, which clips at 1 anyway (an RGBA8 intermediate of tone-mapped linear light would band).  Perceptual
-  // values take the same rule: RCAS's P^-1 squares them, and an RGBA8 intermediate would quantise them like a gamma-2.0
-  // 8-bit image before the sRGB encode.
-  p.midFormat = !srtm && !perceptual ? c->outFormat : (unormOut ? OVRFSR_FORMAT_RGBA16F : OVRFSR_FORMAT_RGBA32F);
-  // OVRFSR_FLAG_FINITE changes no pass and no format, only each pass's bits: finite-in on every pass that reads a float
-  // image, finite-out on every pass that stores one (a UNORM store ignores it, so EASU and NIS always get both).  RCAS
-  // reads the float eye when it runs alone, and EASU's intermediate when that is a float image (a float output, or SRTM);
-  // the paired RCAS reads a UNORM intermediate.  The fused kernel reads the eye and stores UNORM.
-  p.fusedFinite = 0;
-  if ((c->cfg.flags & OVRFSR_FLAG_FINITE) && floatSrc) {
-    const int both = OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_FINITE_OUT;
-    const bool rcasFloatSrc = !p.upscale || p.midFormat == OVRFSR_FORMAT_RGBA16F || p.midFormat == OVRFSR_FORMAT_RGBA32F;
-    p.easuSrtm |= both;
-    p.rcasSrtm |= rcasFloatSrc ? both : 0;
-    p.nisSrtm |= both;
-    p.fusedFinite = OVRFSR_PASS_FINITE_IN;
-  }
+  c->plan = make_plan(c->cfg, src->format, c->outFormat);
+  const Plan &p = c->plan;
   const bool one = c->textureContainsOnlyOneEye;
   const int neyes = one ? 2 : 1;
   for (int e = 0; e < neyes; ++e) {
@@ -483,13 +408,13 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
   // the fused kernel has no array I/O: with an array source or destination the two dispatches run
   if (p.tryFused && !src->array && !fin.array) {
     // EASU and RCAS as one kernel; shapes it does not cover take the two dispatches below
-    e = L.fsr_fused(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev, p.fusedFinite);
+    e = L.fsr_fused(in, finPass, c->upscaleConstants[eye], c->sharpenConstants[eye], s, centreDev, p.easuMaps);
     if (e == cudaSuccess) fused = true;
     else if (e != cudaErrorInvalidValue && e != cudaErrorInvalidConfiguration) return fail(c, OVRFSR_ERR_CUDA, "fused EASU+RCAS launch", e);
   }
   if (p.nis) {
     e = (p.upscale ? L.nis_scaler : L.nis_sharpen)(in, finPass, p.upscale ? c->nisScalerConfig[eye] : c->nisSharpenConfig[eye], s,
-                                                    centreDev, p.nisSrtm);
+                                                    centreDev, p.nisMaps);
     if (e != cudaSuccess)
       return fail(c, (e == cudaErrorInvalidConfiguration || e == cudaErrorInvalidValue) ? OVRFSR_ERR_UNSUPPORTED : OVRFSR_ERR_CUDA,
                   p.upscale ? "NIS scaler dispatch" : "NIS sharpen dispatch", e);
@@ -500,11 +425,11 @@ int apply_post_process(ovrfsr_ctx *c, int eye, const Image *src, Image *out, con
         return fail(c, OVRFSR_ERR_NOMEM, "allocating upscaled texture", cudaGetLastError());
       const PassImage *direct = p.paired ? &finPass : nullptr;
       const float tint = 1.0f - (float)c->sharpenConstants[eye][3] * 0.3f;
-      e = L.easu(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuSrtm);
+      e = L.easu(in, pass_image(up.img), c->upscaleConstants[eye], s, direct, tint, centreDev, p.easuMaps);
       if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "EASU launch", e);
       in = pass_image(up.img);
     }
-    e = L.rcas(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasSrtm);
+    e = L.rcas(in, finPass, c->sharpenConstants[eye], s, p.paired, centreDev, p.rcasMaps);
     if (e != cudaSuccess) return fail(c, OVRFSR_ERR_CUDA, "RCAS launch", e);
   }
   if (q >= 0) { cudaEventRecord(c->evEnd[q], s); c->evPending[q] = true; }
@@ -904,9 +829,7 @@ static int check_nis_image(const Image *im, bool isDst) {
 
 // the pass flags of a stateless dispatch: OVRFSR_OK, or the status to return (checked after the images)
 static int check_pass_flags(const Image *src, int pass_flags) {
-  if (pass_flags & ~(OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_SRTM_OUT | OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_FINITE_OUT |
-                     OVRFSR_PASS_PERCEPTUAL_IN | OVRFSR_PASS_PERCEPTUAL_OUT))
-    return OVRFSR_ERR_INVALID;
+  if (pass_flags & ~(kMapsIn | kMapsOut)) return OVRFSR_ERR_INVALID;
   if (pass_flags && src->format != OVRFSR_FORMAT_RGBA16F && src->format != OVRFSR_FORMAT_RGBA32F) return OVRFSR_ERR_UNSUPPORTED;
   return OVRFSR_OK;
 }

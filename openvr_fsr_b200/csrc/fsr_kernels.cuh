@@ -41,9 +41,9 @@ struct EasuArgs {
   // intermediate `dst` only where an edge-adjacent group is inside the radius (RCAS reads one pixel across the edge).
   ImageRW direct;           // ptr == nullptr: plain dispatch
   float tintGB;             // 1 - debug*0.3 of the following RCAS pass
-  // float sources only, OVRFSR_PASS_* bits (map_in / map_out): srtmIn = SRTM_IN | FINITE_IN | PERCEPTUAL_IN on every
-  // texel read, srtmOut = SRTM_OUT | FINITE_OUT | PERCEPTUAL_OUT on every pixel stored
-  int srtmIn, srtmOut;
+  // float sources only, the per-texel maps (kernels.h): kMapsIn bits on every texel read, kMapsOut bits on every pixel
+  // stored (map_in / map_out)
+  int mapsIn, mapsOut;
 };
 
 struct RcasArgs {
@@ -56,7 +56,7 @@ struct RcasArgs {
   uint32_t radiusSq;
   int skipOutside;          // the preceding EASU launch already wrote the outside-radius groups to dst (EasuArgs::direct)
   int opaqueSrc;            // B8G8R8X8 source: the X byte reads as alpha 1 (only the outside-radius copy looks at alpha)
-  int srtmIn, srtmOut;      // float sources only: OVRFSR_PASS_* bits of the texels read / the pixels stored, as EasuArgs
+  int mapsIn, mapsOut;      // float sources only: the per-texel maps of the texels read / the pixels stored, as EasuArgs
 };
 
 // out pixel -> source position; the same instruction sequence is used for the tile origin and
@@ -487,9 +487,7 @@ __global__ void __launch_bounds__(kThreads, easu_min_ctas(TW)) easu_kernel(const
       const int ty = (int)__umulhi((uint32_t)q, colsRcp), tx = q - ty * cols;
       const int gy = clampi(sy0 + ty, 0, a.src.h - 1), gx = clampi(tx0 + tx, 0, a.src.w - 1);
       float4 c = get_texel<FIN, ANYIO>(a.src, io.src, gx, gy);
-      if constexpr (!packed32(FIN)) {
-        map_in(a.srtmIn, c); // the tile, the features and the bilinear fallback all see F(finite_in(texel))
-      }
+      map_in<FIN>(a.mapsIn, c); // the tile, the features and the bilinear fallback all see the mapped texel
       sL[ty * TW + tx] = c.z * 0.5f + (c.x * 0.5f + c.y);
       c.w = 1.0f; // EASU ignores source alpha; the fast path accumulates the tap weight through this lane
       sC[ty * TW + tx] = c;
@@ -576,7 +574,7 @@ __global__ void __launch_bounds__(kThreads, easu_min_ctas(TW)) easu_kernel(const
         float3 c;
         if constexpr (kStrict) c = easu_filter<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
         else c = easu_filter_fast<TW>(sC + o, sF + o, ppx, ppy_full - fpy);
-        if constexpr (!packed32(FIN)) map_out<FOUT>(a.srtmOut, c.x, c.y, c.z);
+        map_out<FIN, FOUT>(a.mapsOut, c.x, c.y, c.z);
         if constexpr (ANYIO) {
           put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
         } else {
@@ -593,7 +591,7 @@ __global__ void __launch_bounds__(kThreads, easu_min_ctas(TW)) easu_kernel(const
         float3 c = easu_bilinear(sC, TW, ax, sRowAxis[y - oy0]);
         // SRTM_OUT and PERCEPTUAL_OUT never come with `direct` (the launcher rejects them on a paired launch), and
         // FINITE_OUT does nothing there: `direct` is a UNORM target
-        if constexpr (!packed32(FIN)) map_out<FOUT>(a.srtmOut, c.x, c.y, c.z);
+        map_out<FIN, FOUT>(a.mapsOut, c.x, c.y, c.z);
         if (mid) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
         if constexpr (direct) {
           if (a.tintGB == 1.0f) {
@@ -810,8 +808,9 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
         }
         if constexpr (OPQ) c.w = 1.0f;
         // FsrRcasInputF, the hook the reference leaves empty.  The zeros outside the image need no map: F(+0) = +0.
-        // finite_in before the one-colour test, which then compares the mapped texels
-        if constexpr (!packed32(FIN)) map_in(a.srtmIn, c);
+        // finite_in before the one-colour test, which then compares the mapped texels.  The guard repeats map_in's:
+        // without it the UNORM-source instantiations (whose map_in is empty) get other registers.
+        if constexpr (!packed32(FIN)) map_in<FIN>(a.mapsIn, c);
       }
       sC[ty * kRcasTW + tx] = c;
     }
@@ -838,7 +837,7 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       if (y >= a.dst.h) break;
       const float4 h = p[kRcasTW], d = p[-1], f = p[1];
       float3 c = rcas_filter_mode<FIN == OVRFSR_FORMAT_RGBA8 || FIN == OVRFSR_FORMAT_BGRA8>(b, d, e, f, h, sharp);
-      if constexpr (!packed32(FIN)) map_out<FOUT>(a.srtmOut, c.x, c.y, c.z); // also the value a one-colour group's other rows take
+      map_out<FIN, FOUT>(a.mapsOut, c.x, c.y, c.z); // also the value a one-colour group's other rows take
       if constexpr (ANYIO) put_opaque<FOUT, ANYIO>(a.dst, io.dst, x, y, c.x, c.y, c.z);
       else *reinterpret_cast<texel_t<FOUT> *>(out) = encode_opaque<FOUT>(c.x, c.y, c.z);
       if (k == 0 && flat) {
@@ -879,12 +878,14 @@ __global__ void __launch_bounds__(kThreads, 2) rcas_kernel(const __grid_constant
       if (y >= a.dst.h) break;
       const float4 e = p[k * kRcasTW];
       float r = 1.0f * e.x, g = a.tintGB * e.y, bl = a.tintGB * e.z, al = 1.0f * e.w;
+      // What put_mapped does, spelled out: with the channels passed to it as call arguments, or with map_out called
+      // outside this guard, the UNORM-source instantiations get other registers.
       if constexpr (!packed32(FIN)) {
         // the copy runs in the mapped space: G(P^-1(tint x P(F(texel)))), alpha untouched by the maps but clamped by
         // finite_out
-        map_out<FOUT>(a.srtmOut, r, g, bl);
+        map_out<FIN, FOUT>(a.mapsOut, r, g, bl);
         if constexpr (!packed32(FOUT)) {
-          if (a.srtmOut & OVRFSR_PASS_FINITE_OUT) al = finite_out<FOUT>(al);
+          if (a.mapsOut & OVRFSR_PASS_FINITE_OUT) al = finite_out<FOUT>(al);
         }
       }
       put_texel<FOUT, ANYIO>(a.dst, io.dst, x, y, r, g, bl, al);

@@ -15,6 +15,12 @@ struct PassImage { void *ptr; uint32_t pitch; int w, h; int format; bool array =
 // the `centreDev` block described below: its size in words and where its sharpness words sit
 constexpr int kLatchWords = 16, kLatchRcasSharp = 6, kLatchNisSharp = 8;
 
+// The per-texel maps of a pass (`maps` below): OVRFSR_PASS_* bits of the texels it reads and of the pixels it stores.
+// Read order finite-in, SRTM's F, perceptual P; store order P^-1, G, finite-out or the sRGB encode (device_common.cuh,
+// map_in / map_out).  The maps are defined for float sources only.
+constexpr int kMapsIn = OVRFSR_PASS_SRTM_IN | OVRFSR_PASS_FINITE_IN | OVRFSR_PASS_PERCEPTUAL_IN;
+constexpr int kMapsOut = OVRFSR_PASS_SRTM_OUT | OVRFSR_PASS_FINITE_OUT | OVRFSR_PASS_PERCEPTUAL_OUT;
+
 // The launchers of one math mode, one per pass: kernels_fast.cu fills kFastLaunchers, kernels_strict.cu kStrictLaunchers.
 struct Launchers {
   // FSR (fsr_kernels.cuh).  consts are the reference's constant-buffer layouts.
@@ -28,26 +34,24 @@ struct Launchers {
   //   words 0-3 imageCentre, 4-5 radiusSq of centre pair 0 / 1, 6 RCAS const0[0] (RCAS and the fused kernel),
   //   8-9 NISConfig kSharpStrengthMin / kSharpStrengthScale, 10-11 kSharpLimitMin / kSharpLimitScale (NVScaler and
   //   NVSharpen), 7 and 12-15 padding.  EASU reads words 0-5 only.
-  // `srtm` (EASU and RCAS): OVRFSR_PASS_SRTM_* bits, AMD's reversible tone map on the texels read / the pixels stored,
-  // OR-ed with OVRFSR_PASS_FINITE_* (OVRFSR_FLAG_FINITE) and OVRFSR_PASS_PERCEPTUAL_* (OVRFSR_FLAG_PERCEPTUAL).  Float
-  // sources only, and the SRTM and perceptual bits never together with the pairing: cudaErrorInvalidValue otherwise.
+  // `maps` (every launcher but CAS): kMapsIn | kMapsOut bits.  Any bit with a UNORM source, or a bit the pass does not
+  // take, is cudaErrorInvalidValue.  EASU with `direct` takes only the finite bits (finite-out does nothing to its UNORM
+  // stores), RCAS with `skipOutside` none: the pairing copies UNORM codes, which mapped values are not.
   cudaError_t (*easu)(const PassImage &src, const PassImage &dst, const uint32_t consts[24], cudaStream_t s,
-                      const PassImage *direct, float tintGB, const uint32_t *centreDev, int srtm);
+                      const PassImage *direct, float tintGB, const uint32_t *centreDev, int maps);
   cudaError_t (*rcas)(const PassImage &src, const PassImage &dst, const uint32_t consts[12], cudaStream_t s,
-                      bool skipOutside, const uint32_t *centreDev, int srtm);
+                      bool skipOutside, const uint32_t *centreDev, int maps);
   // EASU -> RCAS in one kernel (fsr_fused.cuh): ku = UpscaleConstants, ks = SharpenConstants; dst.format (RGBA8, or
   // RGB10A2 for an RGB10A2 source) is also the format the intermediate is quantised to.  cudaErrorInvalidValue /
   // cudaErrorInvalidConfiguration = this pair of passes cannot be fused (the caller runs the two dispatches instead).
-  // `finite`: finite-in of OVRFSR_FLAG_FINITE on every texel read (float sources only; the target is UNORM).
+  // `maps`: the finite bits only; finite-in on every texel read, and finite-out does nothing to the UNORM target.
   cudaError_t (*fsr_fused)(const PassImage &src, const PassImage &dst, const uint32_t ku[24], const uint32_t ks[12],
-                           cudaStream_t s, const uint32_t *centreDev, int finite);
-  // NIS (nis_kernels.cuh), with this library's filter banks.  cfg256 = the 256-byte NISConfig block.  `srtm`:
-  // OVRFSR_PASS_SRTM_* / _FINITE_* / _PERCEPTUAL_* bits as for EASU and RCAS (OVRFSR_FLAG_SRTM_NIS, OVRFSR_FLAG_FINITE,
-  // OVRFSR_FLAG_PERCEPTUAL).  Float sources only: cudaErrorInvalidValue otherwise.
+                           cudaStream_t s, const uint32_t *centreDev, int maps);
+  // NIS (nis_kernels.cuh), with this library's filter banks.  cfg256 = the 256-byte NISConfig block.
   cudaError_t (*nis_scaler)(const PassImage &src, const PassImage &dst, const void *cfg256, cudaStream_t s,
-                            const uint32_t *centreDev, int srtm);
+                            const uint32_t *centreDev, int maps);
   cudaError_t (*nis_sharpen)(const PassImage &src, const PassImage &dst, const void *cfg256, cudaStream_t s,
-                             const uint32_t *centreDev, int srtm);
+                             const uint32_t *centreDev, int maps);
   // legacy CAS (cas_kernels.cuh).  consts = const0, const1 of src/cas/cas.compute.h:1-4 as CasSetup fills them.
   cudaError_t (*cas)(const PassImage &src, const PassImage &dst, const uint32_t consts[8], int sharpenOnly, cudaStream_t s);
 };
