@@ -113,23 +113,27 @@ def _source(src, src_fmt):
     return so._float_source(src)
 
 
-def easu(src, out_w, out_h, consts, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None):
-    o = _EASU(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), out_w, out_h, consts, out_dtype=np.float32)
+def easu(src, out_w, out_h, consts, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None, nthreads=1):
+    o = _EASU(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), out_w, out_h, consts, out_dtype=np.float32,
+              nthreads=nthreads)
     return store(o, bits, out_dtype, dst_fmt)
 
 
-def rcas(src, consts, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None):
-    o = _RCAS(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), consts, out_dtype=np.float32)
+def rcas(src, consts, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None, nthreads=1):
+    o = _RCAS(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), consts, out_dtype=np.float32,
+              nthreads=nthreads)
     return store(o, bits, out_dtype, dst_fmt)
 
 
-def nis_scaler(src, out_w, out_h, cfg, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None):
-    o = _NIS_SCALER(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), out_w, out_h, cfg, out_dtype=np.float32)
+def nis_scaler(src, out_w, out_h, cfg, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None, nthreads=1):
+    o = _NIS_SCALER(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), out_w, out_h, cfg,
+                    out_dtype=np.float32, nthreads=nthreads)
     return store(o, bits, out_dtype, dst_fmt)
 
 
-def nis_sharpen(src, cfg, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None):
-    o = _NIS_SHARPEN(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), cfg, out_dtype=np.float32)
+def nis_sharpen(src, cfg, out_dtype=np.uint8, bits=0, src_fmt=None, dst_fmt=None, nthreads=1):
+    o = _NIS_SHARPEN(np.ascontiguousarray(read_map(_source(src, src_fmt), bits)), cfg, out_dtype=np.float32,
+                    nthreads=nthreads)
     return store(o, bits, out_dtype, dst_fmt)
 
 
@@ -153,6 +157,18 @@ def ctx_bits(flags, nis, upscale, unorm_out):
         rcas_b |= both if (not upscale or mid is not None or not unorm_out) else 0
         nis_b |= both
     return easu_b, rcas_b, nis_b, mid
+
+
+def ctx_plan(flags, nis, upscale, src_fmt, out_fmt):
+    """the rest of the plan (csrc/plan.h, make_plan) from ctx_bits, for an ovrfsr_format source src_fmt and the output
+    format out_fmt prepare_resources accepted: (easu, rcas, nis bits, intermediate dtype or None for the output's
+    format, paired, fused tried, sRGB-encoded output).  A UNORM source gets no bits; the pairing needs a UNORM output
+    and an intermediate in its format; the output is sRGB-encoded for PERCEPTUAL with a float source into RGBA8."""
+    float_src = src_fmt in (2, 3, 6)  # RGBA16F, RGBA32F, RGB32F
+    unorm_out = out_fmt in (0, 4)     # RGBA8, RGB10A2
+    easu_b, rcas_b, nis_b, mid = ctx_bits(flags, nis, upscale, unorm_out) if float_src else (0, 0, 0, None)
+    paired = not nis and upscale and unorm_out and mid is None
+    return easu_b, rcas_b, nis_b, mid, paired, paired and bool(flags & 1), float_src and bool(flags & 16) and out_fmt == 0
 
 
 def fsr_chain(src, uc, sc, out_w, out_h, out_dtype, flags, upscale=True, src_fmt=None):

@@ -1,11 +1,12 @@
 """The context's pass plan without a GPU: make_plan (csrc/plan.h, what prepare_resources runs) for every use_nis, render
 scale 1 and 0.75, output format, source format and flags 0..31 that prepare_resources accepts, against the statement the
-GPU tests check the context path with (perceptual_oracle.ctx_bits) and the rules of include/ovrfsr.h."""
+GPU tests check the context path with (perceptual_oracle.ctx_bits and ctx_plan) and the rules of include/ovrfsr.h."""
 import shutil
 import subprocess
 import tempfile
 from pathlib import Path
 
+import numpy as np
 import pytest
 
 from tests import perceptual_oracle as pq
@@ -61,4 +62,11 @@ def test_make_plan_states_the_rule():
         got = dict(easu=easu, rcas=rcas, nis=nis_b)
         for name in ("easu", "rcas", "nis"):
             assert got[name] == (want[name] if name in runs else 0), (name, where)
+        # the whole plan as tests/test_gpu_frame_fuzz.py takes it from the checker's one statement
+        e, r, n, pmid, ppaired, pfused, psrgb = pq.ctx_plan(flags, bool(nis), bool(upscale), src, out)
+        assert (ppaired, pfused, psrgb) == (bool(paired), bool(fused), bool(srgb)), where
+        if not nis and upscale:
+            assert mid == {None: out, np.float16: RGBA16F, np.float32: RGBA32F}[pmid], where
+        for name, bits in (("easu", e), ("rcas", r), ("nis", n)):
+            assert got[name] == (bits if name in runs else 0), (name, where)
     assert checked == 2 * 2 * 32 * 7 * 4  # each source: AUTO, its UNORM output and the two float outputs
