@@ -221,9 +221,18 @@ __device__ __forceinline__ float3 easu_filter_fast(const float4 *__restrict__ cf
   dir = fma2(make_float2(Fk.x, Fk.y), bc(wb.y), dir); ln = fma2(make_float2(Fk.z, Fk.w), bc(wb.y), ln);
   float len = ln.x + ln.y;
 
+  // The branch (:389-395) is decided on dir^2 as easu_filter forms it, every product and sum rounded on its own: zro
+  // turns the kernel by up to 90 degrees, so the FMA-blended dir^2 above, an ulp or two away from the reference's,
+  // takes the other branch where dir^2 sits on 2^-15 (tests/test_gpu_easu_direction.py).  Only the decision: the
+  // direction that is normalised stays the FMA blend, so every pixel whose branch the FMA blend already took the
+  // reference's way keeps the bits it had.
+  const float rdx = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(Ff.x, wt.x), __fmul_rn(Fg.x, wt.y)), __fmul_rn(Fj.x, wb.x)),
+                              __fmul_rn(Fk.x, wb.y));
+  const float rdy = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(Ff.y, wt.x), __fmul_rn(Fg.y, wt.y)), __fmul_rn(Fj.y, wb.x)),
+                              __fmul_rn(Fk.y, wb.y));
+  const bool zro = __fadd_rn(__fmul_rn(rdx, rdx), __fmul_rn(rdy, rdy)) < (float)(1.0 / 32768.0);
   f2 dd = mul2(dir, dir);
   float dirR = dd.x + dd.y;
-  const bool zro = dirR < (float)(1.0 / 32768.0);
   dirR = zro ? 1.0f : prx_lo_rsq(dirR);
   dir.x = zro ? 1.0f : dir.x;
   dir = mul2(dir, bc(dirR));
