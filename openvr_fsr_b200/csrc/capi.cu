@@ -14,6 +14,7 @@
 #include "array_io.h"
 #include "host_constants.h"
 #include "kernels.h"
+#include "launch.cuh"
 #include "nis_host.h"
 #include "plan.h"
 
@@ -84,9 +85,8 @@ __global__ void __launch_bounds__(256) repitch_rows_kernel(uint8_t *__restrict__
 cudaError_t repitch_rows(void *dst, size_t dpitch, const void *src, size_t spitch, size_t rowBytes, uint32_t rows, cudaStream_t s) {
   const uint32_t rowWords = (uint32_t)(rowBytes / 4);
   dim3 grid((rowWords + 1023) / 1024, rows < 4096 ? rows : 4096);
-  repitch_rows_kernel<<<grid, 256, 0, s>>>(static_cast<uint8_t *>(dst), dpitch, static_cast<const uint8_t *>(src), spitch, rowWords, rows);
-  count_launch();
-  return cudaGetLastError();
+  return launch<repitch_rows_kernel>(grid, 256, 0, kNoOptIn, s, static_cast<uint8_t *>(dst), dpitch, static_cast<const uint8_t *>(src),
+                                     spitch, rowWords, rows);
 }
 
 // R32G32B32_FLOAT -> RGBA32F, alpha 1 (a three-component view reads 1 in .w)
@@ -99,10 +99,8 @@ __global__ void __launch_bounds__(256) expand_rgb32f_kernel(float4 *__restrict__
 }
 cudaError_t expand_rgb32f(const ovrfsr_image &src, const ovrfsr_image &dst, cudaStream_t s) {
   const dim3 grid((src.width + 255) / 256, src.height);
-  expand_rgb32f_kernel<<<grid, 256, 0, s>>>(static_cast<float4 *>(dst.data), dst.pitch, static_cast<const float *>(src.data), src.pitch,
-                                              src.width, src.height);
-  count_launch();
-  return cudaGetLastError();
+  return launch<expand_rgb32f_kernel>(grid, 256, 0, kNoOptIn, s, static_cast<float4 *>(dst.data), dst.pitch,
+                                       static_cast<const float *>(src.data), src.pitch, src.width, src.height);
 }
 
 // The radius mask's focus and radius and the sharpness (ovrfsr_set_focus, ovrfsr_set_focus_radius,

@@ -69,7 +69,4 @@ cudaError_t selftest_nis_div(uint32_t result[2], cudaStream_t s);
 // `samples` consecutive samples of each texel; same format both sides.  One arithmetic (strict) for both math modes.
 cudaError_t launch_resolve_msaa(const PassImage &srcSamples, int samples, const PassImage &dst, cudaStream_t s);
 
-// bumped once per kernel launch by every launcher (ovrfsr_kernel_launches)
-void count_launch();
-
 } // namespace ovrfsr
